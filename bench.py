@@ -3,11 +3,12 @@
 
   python bench.py --gpus N --steps K --warmup W            our arm (one rank per GPU under torchrun for N > 1)
   python bench.py --impl reference --gpus N --steps K ...  the reference's CPU algorithm (oracle port, all host threads)
+  python bench.py ... --dump-outputs DIR                   also write what the last timed step computed as DIR/<name>.npy
 
 A "step" is ONE hot-path SQP iteration (SURVEY.md 8d) for every OCP of the batch, given the stage linearisations
 resident in HBM:  condense (PDIPM + contact/impact dynamics + SE(3) state-equation correction)  ->  backward Riccati
 ->  forward Riccati  ->  primal expansion + fraction-to-boundary step sizes  ->  dual expansion + primal/dual update
-(the linear-algebra body of OCPSolver::updateSolution, /root/reference/src/solver/ocp_solver.cpp:118-144).
+(the linear-algebra body of OCPSolver::updateSolution, robotoc's src/solver/ocp_solver.cpp:118-144).
 Weak scaling: every GPU owns `--batch` OCPs (instances are independent); with N > 1 the Newton step is all-gathered once
 per step over NCCL.  Prints ONE JSON line (rank 0).  PyTorch is plumbing only (streams, events, pinned memory,
 torch.distributed).
@@ -18,6 +19,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -41,21 +43,6 @@ BYTES_PER_STAGE_MJTJINV = (324 + 216 + 900) * 8               # K1 reads M, J an
 BYTES_PER_STAGE_ITERATION = int((69.2 + 45.6 + 5.0) * 1000) - 2 * (1620 - 666) * 8
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum (bytes per launch at batch 1024) of the committed `ncu --set full` capture of
-    this very command: profiles/r2_final_<kernel>_ncu_summary.txt."""
-    path = os.path.join(ROOT, "profiles", f"r2_final_{kernel}_kernel_ncu_summary.txt")
-    tot, unit = 0.0, {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-    try:
-        for line in open(path):
-            f = line.split()
-            if len(f) >= 3 and f[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                tot += float(f[1]) * unit[f[2]]
-    except OSError:
-        return None, None
-    return (tot or None), os.path.relpath(path, ROOT)
-
-
 FLOP_PER_STAGE_BWD = 285.7e3
 FLOP_PER_STAGE_CONDENSE = 300e3
 
@@ -69,6 +56,8 @@ def parse():
     ap.add_argument("--batch", type=int, default=1024, help="OCP instances per GPU (BASELINE config 3: 1024)")
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (fixed sample of DUMP_OCPS OCPs) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -105,7 +94,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -212,12 +201,12 @@ def _oracle_runner(pr):
     os.environ.setdefault("OMP_DYNAMIC", "false")
     import oracle_lib
     lib = oracle_lib.load()
-    native = os.path.join(oracle_lib.ORACLE_DIR, "liboracle_native.so")
-    try:  # -march=native build of the same sources, made on this machine
-        # -B: always rebuilt here -- a copy that travelled from another machine was tuned for that machine's CPU
-        subprocess.run(["make", "-s", "-B", "-C", oracle_lib.ORACLE_DIR, "native"], check=True, stdout=subprocess.DEVNULL,
-                       stderr=subprocess.DEVNULL)
-        lib = ct.CDLL(native)
+    try:  # -march=native build of the same sources, made on this machine, in a temporary directory (the tree may be read-only)
+        with tempfile.TemporaryDirectory(prefix="rbt_bench_") as tmp:  # removed once loaded: the mapping outlives the file
+            native = os.path.join(tmp, "liboracle_native.so")
+            subprocess.run(["make", "-s", "-C", oracle_lib.ORACLE_DIR, "native", f"NATIVE={native}"], check=True,
+                           stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+            lib = ct.CDLL(native)
     except Exception:
         pass
     from robotoc_b200._lib import rbt_stage_ctrl
@@ -253,7 +242,7 @@ def _oracle_runner(pr):
 
 
 WORKLOAD = "anymal_trot_N40 batch={b}/GPU: full hot-path iteration = condense + riccati backward + riccati forward + step sizes + update"
-METRIC = "SQP-iterations/s (ANYmal N=40, batch=1024) at 1/2/4/8 B200 vs CPU ref"
+METRIC = "SQP-iterations/s (ANYmal N=40, batch=1024) at 1/2/4/8 H100 vs CPU ref"
 
 
 def bench_config(batch, n_grid, world, l2_note):
@@ -266,7 +255,23 @@ def bench_config(batch, n_grid, world, l2_note):
 def l2_note(pr):
     lin, K = pr["lin"], pr["K"]
     ws = lin.nbytes + lin.shape[0] * lin.shape[1] * (K.k_stride + K.r_stride) * 8
-    return f"per-step working set {ws / 1e9:.2f} GB >> 126 MB L2 (inputs larger than L2; no flush needed)"
+    return f"per-step working set {ws / 1e9:.2f} GB >> 50 MB L2 (inputs larger than L2; no flush needed)"
+
+
+DUMP_OCPS = 256  # OCPs of the batch whose outputs --dump-outputs writes: a fixed, seeded sample keeps the files under 64 MB
+
+
+def dump_outputs(out_dir, S, K, d, sol, con, steps):
+    """What a caller of the timed path receives after one iteration, for DUMP_OCPS OCPs chosen by a fixed seed: the Newton
+    direction records, the used prefix of the updated solution records, the updated slack | dual of the PDIPM records, and the
+    primal / dual step sizes of every OCP."""
+    os.makedirs(out_dir, exist_ok=True)
+    batch = d.shape[0]
+    ocp = np.sort(np.random.default_rng(0).choice(batch, min(batch, DUMP_OCPS), replace=False))
+    arrays = {"direction": d[ocp], "solution": sol[ocp, :, :S.s_xi + S.nsm], "slack_dual": con[ocp, :, :2 * S.ncp],
+              "step_sizes": steps}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def cpu_modes(pr, min_seconds):
@@ -502,6 +507,8 @@ def main():
         assert err < 1e-8, f"rank {rank}: gathered step disagrees with the oracle ({err:.2e})"
     sol_dev = dms.getSolution()
     steps_dev = np.stack([dms.maxPrimalStepSize(), dms.maxDualStepSize()], axis=1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, S, K, d_local.cpu().numpy(), sol_dev, con_work.cpu().numpy(), steps_dev)
 
     # ---- end-to-end arm: host (pinned) buffers through the one-call C-ABI entry point, H2D + D2H inside the timed region
     pin = lambda a: torch.from_numpy(a).pin_memory()  # noqa: E731
@@ -563,11 +570,10 @@ def main():
         alg_bytes = {"riccati_backward": BYTES_PER_STAGE_BWD, "riccati_forward": BYTES_PER_STAGE_FWD,
                      "condense": BYTES_PER_STAGE_CONDENSE}.get(dom, BYTES_PER_STAGE_BWD) * units
         ach = alg_bytes / (kms[dom] * 1e-3) / 1e9
-        traffic, traffic_src = ncu_traffic(dom) if dom in ("condense", "riccati_backward") else (None, None)
         kname = {"riccati_backward": "riccati_backward_kernel<18,12,12>", "condense": "condense_kernel<18,12,12>",
                  "riccati_forward": "riccati_forward_kernel<18,12,12>"}.get(dom, dom)
         line = {
-            "metric": METRIC,
+            "metric": METRIC, "device": torch.cuda.get_device_name(local),
             "value": world * args.batch * args.steps / (ms * 1e-3), "unit": "OCP-iterations/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
@@ -587,8 +593,6 @@ def main():
                             "wire": "rbt_iteration_host_wire (as resident, plus PDIPM slack|dual and the solution uploaded every step)",
                             "dense": "rbt_iteration_host (dense linearisation records)"}[e2e_mode]},
             "roofline": {"bound": "hbm", "kernel": kname, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                         "traffic": (traffic * args.batch / 1024) if traffic else None,
-                         "traffic_source": f"dram__bytes_read + write of the ncu --set full capture of this command ({traffic_src}), per launch",
                          "frac_8d_literal": (BYTES_PER_STAGE_CONDENSE_8D * units / (kms[dom] * 1e-3) / 1e9 / peak) if dom == "condense" else None,
                          "iteration": {"algorithmic_bytes": BYTES_PER_STAGE_ITERATION * units,
                                        "achieved": BYTES_PER_STAGE_ITERATION * units / (ms / args.steps * 1e-3) / 1e9,
@@ -601,7 +605,7 @@ def main():
                              "mjtjinv": BYTES_PER_STAGE_MJTJINV * units / (kms["mjtjinv"] * 1e-3) / 1e9},
                          "fp64_tflops": {"riccati_backward": FLOP_PER_STAGE_BWD * units / (kms["riccati_backward"] * 1e-3) / 1e12,
                                          "condense": FLOP_PER_STAGE_CONDENSE * units / (kms["condense"] * 1e-3) / 1e12},
-                         "fp64_peak_tflops": 37.1},
+                         "fp64_peak_tflops": 67.0, "fp64_peak_source": "H100 SXM data sheet (FP64 tensor core), not measured"},
         }
         if world == 1 and not args.no_cpu_baseline:
             line["cpu_baseline"] = cpu_leg(pr, min_seconds=10.0)

@@ -4,13 +4,13 @@
  * Plain C (usable from gcc, g++ and nvcc).  The records mirror the reference's
  * per-stage containers, block by block, as contiguous column-major doubles:
  *
- *   KKT record      <-> robotoc::SplitKKTMatrix   (/root/reference/src/core/split_kkt_matrix.cpp:7-34)
- *                       robotoc::SplitKKTResidual (/root/reference/src/core/split_kkt_residual.cpp:7-20)
+ *   KKT record      <-> robotoc::SplitKKTMatrix   (robotoc/src/core/split_kkt_matrix.cpp:7-34)
+ *                       robotoc::SplitKKTResidual (robotoc/src/core/split_kkt_residual.cpp:7-20)
  *   Riccati record  <-> robotoc::SplitRiccatiFactorization (include/robotoc/riccati/split_riccati_factorization.hpp),
  *                       robotoc::LQRPolicy (include/robotoc/riccati/lqr_policy.hpp:16-126; K is ROW-major there,
  *                       i.e. the same memory as a column-major nx x nu K^T, which is what we store),
  *                       robotoc::STOPolicy (include/robotoc/riccati/sto_policy.hpp)
- *   Direction record<-> robotoc::SplitDirection   (/root/reference/src/core/split_direction.cpp:7-22)
+ *   Direction record<-> robotoc::SplitDirection   (robotoc/src/core/split_direction.cpp:7-22)
  *
  * Arrays are [batch][stage][record]; every section offset is a multiple of 2 doubles (16 B,
  * the cp.async.bulk granule) and every record stride a multiple of 16 doubles (128 B).
@@ -157,7 +157,7 @@ static inline RBT_HD void rbt_make_layout(const rbt_dims* d, rbt_layout* L) {
 
 /* ---------------- unconstrained (fixed-base, no contacts) path: implicit A=[[I,dt I],[0,I]], B=[0;dt I];
  * control = acceleration a (dim nv).  Mirrors what UnconstrRiccatiRecursion touches
- * (/root/reference/src/riccati/unconstr_riccati_recursion.cpp:26-48): Qxx,Qxu,Qaa,Fx,lx,la. */
+ * (robotoc/src/riccati/unconstr_riccati_recursion.cpp:26-48): Qxx,Qxu,Qaa,Fx,lx,la. */
 typedef struct rbt_ulayout {
   int nv, nx;
   int k_Qxx, k_Qxu, k_Qaa, k_Fx, k_lx, k_la, k_stride;

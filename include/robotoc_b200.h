@@ -1,5 +1,5 @@
 /*
- * robotoc_b200.h -- C ABI of the B200-native Riccati / KKT inner loop (librobotoc_b200.so).
+ * robotoc_b200.h -- C ABI of the H100-native Riccati / KKT inner loop (librobotoc_b200.so).
  *
  * This is the drop-in boundary behind robotoc::OCPSolver / UnconstrOCPSolver.  The reference has no
  * FFI seam; the seam is the C++ member API of its solver classes.  Every entry point below names
@@ -13,7 +13,7 @@
  *    device.  All work is stream-ordered; call rbt_sync() (or synchronise the stream) before reading
  *    host outputs.
  *  - there is NO CPU fallback: every compute entry point fails with RBT_ERR_CUDA if no usable
- *    sm_100 device is present.
+ *    sm_90 device is present.
  */
 #ifndef ROBOTOC_B200_H_
 #define ROBOTOC_B200_H_

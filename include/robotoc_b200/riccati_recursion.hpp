@@ -124,7 +124,7 @@ class RiccatiRecursion {
       const std::string msg = h_ ? rbt_last_error(h_) : "unsupported robot dimensions";
       if (h_) rbt_destroy(h_);
       h_ = nullptr;
-      throw std::runtime_error("[RiccatiRecursion] cannot create the B200 handle: " + msg);
+      throw std::runtime_error("[RiccatiRecursion] cannot create the device handle: " + msg);
     }
     lqr_policy_.assign(n_grid_max, LQRPolicy(dims_.nv, dims_.nu));
   }
@@ -305,7 +305,7 @@ class DeviceRiccatiRecursion {  // batch-of-one-or-more variant that keeps every
     if (rbt_create(&dims_, n_grid_, batch, device, &h_) != RBT_OK) {
       const std::string msg = h_ ? rbt_last_error(h_) : "unsupported robot dimensions";
       if (h_) rbt_destroy(h_);
-      throw std::runtime_error("[RiccatiRecursion] cannot create the B200 handle: " + msg);
+      throw std::runtime_error("[RiccatiRecursion] cannot create the device handle: " + msg);
     }
     const int rc = rbt_set_schedule(h_, ctrl.data(), n_grid_, max_dts0);
     if (rc != RBT_OK) {  // the destructor does not run when a constructor throws: release the handle here

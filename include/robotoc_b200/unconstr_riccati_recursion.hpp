@@ -55,7 +55,7 @@ class UnconstrRiccatiRecursion {
       const std::string msg = h_ ? rbt_unconstr_last_error(h_) : "unsupported robot dimension";
       if (h_) rbt_unconstr_destroy(h_);
       h_ = nullptr;
-      throw std::runtime_error("[UnconstrRiccatiRecursion] cannot create the B200 handle: " + msg);
+      throw std::runtime_error("[UnconstrRiccatiRecursion] cannot create the device handle: " + msg);
     }
     lqr_policy_.assign(size_t(N) + 1, UnconstrLQRPolicy(nv));
   }

@@ -4,7 +4,7 @@
  * primal / dual expansion, fraction-to-boundary step sizes and the primal/dual update.
  *
  * Plain-C restatement of the reference (robotoc @ d30d404), every function citing the lines it follows.
- * PARITY STATUS: PINNED against the reference's own code.  /root/reference/src/dynamics/{contact_dynamics,impact_dynamics,
+ * PARITY STATUS: PINNED against the reference's own code.  robotoc/src/dynamics/{contact_dynamics,impact_dynamics,
  * state_equation,impact_state_equation,terminal_state_equation,...}.cpp, src/constraints/{constraints,friction_cone,joint_*_limit,
  * constraint_component_*}.cpp and src/core are compiled UNMODIFIED (oracle/Makefile.ref, Eigen / Robot stand-ins of oracle/shim)
  * and driven stage by stage in the order Intermediate/Impact/TerminalStage use them (oracle/ref_wrap/ref_stage_wrap.cpp);

@@ -1,5 +1,5 @@
 // oracle/ref_wrap/ref_riccati_wrap.cpp -- TEST INFRASTRUCTURE.  C entry points around the REFERENCE's own Riccati classes,
-// compiled unmodified from /root/reference/src/riccati/*.cpp and src/core/split_*.cpp (see oracle/Makefile.ref) against the
+// compiled unmodified from robotoc/src/riccati/*.cpp and src/core/split_*.cpp (see oracle/Makefile.ref) against the
 // Eigen / Robot stand-ins of oracle/shim/.  Records in and out use the packed layout of include/rbt_layout.h, exactly like
 // the oracle's orc_riccati_batch / orc_unconstr_batch, so a test can hand the same arrays to both and compare.
 //   robotoc::RiccatiRecursion::backwardRiccatiRecursion / forwardRiccatiRecursion   src/riccati/riccati_recursion.cpp:32-131

@@ -1,5 +1,5 @@
 // oracle/ref_wrap/ref_stage_wrap.cpp -- TEST INFRASTRUCTURE.  One OCP stage through the REFERENCE's own stage-layer code
-// (compiled unmodified from /root/reference/src/dynamics, src/constraints, src/core; oracle/Makefile.ref), in the order
+// (compiled unmodified from robotoc/src/dynamics, src/constraints, src/core; oracle/Makefile.ref), in the order
 // {Intermediate,Impact}Stage use it (src/ocp/intermediate_stage.cpp:133-203, impact_stage.cpp:115-169):
 //   Constraints::condenseSlackAndDual -> condenseContactDynamics | condenseImpactDynamics -> correctLinearize(Impact)StateEquation
 //   -> [STO scaling of intermediate_stage.cpp:140-148, seven scalings restated here: they are lines of a member function that

@@ -5,12 +5,12 @@
  * (robotoc @ d30d404).  Nothing in the product path (robotoc_b200/, include/) may
  * call into this file; only tests/, __graft_entry__.smoke() and bench.py's CPU legs do.
  *
- * PARITY STATUS: PINNED against the reference's own code.  /root/reference/src/riccati/ (all .cpp files) and src/core/split_{kkt_matrix,kkt_residual,direction}.cpp are
+ * PARITY STATUS: PINNED against the reference's own code.  robotoc/src/riccati/ (all .cpp files) and src/core/split_{kkt_matrix,kkt_residual,direction}.cpp are
  * compiled UNMODIFIED (oracle/Makefile.ref) against a self-written stand-in for the Eigen3 / Robot API (oracle/shim/) into
  * oracle/_ref/libref_riccati.so; tests/test_golden_ref.py compares this file with that library on every field of every
  * Riccati / direction record and of the mutated KKT blocks (event schedules with and without switching-time optimisation,
  * BASELINE trot N=40 and jump STO N=80, iiwa14): agreement 1e-15 .. 3e-15.  tests/golden/golden_ref_r2.npz holds outputs of
- * that library (tests/golden/make_golden_ref.py), so the pin also holds on the GPU box where /root/reference does not exist.
+ * that library (tests/golden/make_golden_ref.py), so the pin also holds where no robotoc tree is available.
  * Besides: the reference tests' algebraic identities re-run with fixed seeds and an independent dense solve of the full block
  * KKT system in numpy (tests/test_oracle_kkt.py; for the STO path with the switching-time increments as unknowns: exact up to
  * the three places where the reference itself departs from the exact Newton step, all restated here and documented at

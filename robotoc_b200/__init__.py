@@ -1,8 +1,8 @@
-"""robotoc_b200 -- B200-native (sm_100a) Riccati / KKT inner loop behind robotoc's OCPSolver API.
+"""robotoc_b200 -- H100-native (sm_90a) Riccati / KKT inner loop behind robotoc's OCPSolver API.
 
 Host-side Python mirror of the reference interface for the hot path only (SURVEY.md section 8):
-  RiccatiRecursion / UnconstrRiccatiRecursion  <-> /root/reference/include/robotoc/riccati/*.hpp
-  TimeDiscretization (control table producer)  <-> /root/reference/src/ocp/time_discretization.cpp
+  RiccatiRecursion / UnconstrRiccatiRecursion  <-> robotoc/include/robotoc/riccati/*.hpp
+  TimeDiscretization (control table producer)  <-> robotoc/src/ocp/time_discretization.cpp
 All compute goes through the C ABI of librobotoc_b200.so (include/robotoc_b200.h); there is no CPU path.
 """
 from .layout import Dims, Layout, ULayout  # noqa: F401

@@ -130,7 +130,7 @@ static bool instance_supported(const rbt_dims& d) {
 
 // All functions below are declared extern "C" in include/robotoc_b200.h; the definitions inherit that linkage.
 
-const char* rbt_version(void) { return "robotoc_b200 0.1 (sm_100a; instances: constrained nv18/nu12/ns12; unconstr nv7)"; }
+const char* rbt_version(void) { return "robotoc_b200 0.1 (sm_90a; instances: constrained nv18/nu12/ns12; unconstr nv7)"; }
 
 int rbt_layout_get(const rbt_dims* dims, const char* field) {
   if (!dims || !field) return -1;

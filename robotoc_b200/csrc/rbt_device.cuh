@@ -1,7 +1,6 @@
-// rbt_device.cuh -- sm_100a device helpers: 1-D TMA bulk copies + mbarrier, fp64 tensor-pipe tiles
-// (mma.sync.m8n8k4.f64, DMMA), small warp-parallel dense helpers.  fp64 has no tcgen05 kind, so the
-// tensor pipe is reached through DMMA; measured on B200: 37.1 TFLOP/s DMMA vs 33.5 DFMA vs ~18 for
-// shared-memory-fed DFMA (gpurun_out/fp64_microbench.txt, tools/fp64_microbench.cu).
+// rbt_device.cuh -- sm_90a device helpers: 1-D TMA bulk copies + mbarrier, fp64 tensor-pipe tiles
+// (mma.sync.m8n8k4.f64, DMMA), small warp-parallel dense helpers.  fp64 has no wgmma kind, so the
+// tensor pipe is reached through DMMA (tools/fp64_microbench.cu compares it with DFMA).
 #pragma once
 #include <cstdint>
 #include <cstdio>
@@ -89,14 +88,14 @@ __host__ __device__ constexpr int num_tiles(int M) { return (M + 7) / 8; }
 //   fa(i, k) / fb(k, j) return the operand element (shared-memory loads).  K need not be a multiple of 4.
 // n_begin (warp-uniform): tiles n < n_begin are skipped (symmetric products: only the tiles on/above the diagonal band).
 // PIPE = false: one fragment set, the loads of k-step ks issued right before its MMAs (NT + 1 fewer live doubles) -- for the
-// register-starved backward sweep (80-register cap: the second fragment set only adds spills there; measured 4.5 % faster).
+// register-starved backward sweep (80-register cap: the second fragment set only adds spills there).
 template <int K, int NT, int N, bool PIPE = true, class FA, class FB>
 __device__ __forceinline__ void warp_mma_band(double (&acc)[NT][2], int i0, FA fa, FB fb, int n_begin = 0) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   constexpr int KS = (K + 3) / 4;
   // Software-pipelined by hand: the operands of k-step ks+1 are loaded BEFORE the NT tensor instructions of k-step ks are
   // issued.  (The volatile MMA statements are scheduling barriers for ptxas: with the natural "load b, mma, load b, mma"
-  // order every DMMA waited a full shared-memory latency for its own operand -- ~65 cycles per DMMA instead of 16.)
+  // order every DMMA would wait a full shared-memory latency for its own operand.)
   auto load = [&](int ks, double& a, double (&b)[NT]) {
     const int k0 = 4 * ks;
     // K tail: load from a clamped (valid) index and zero the A operand arithmetically -- no per-thread branch
@@ -209,8 +208,8 @@ __device__ __forceinline__ double fast_rsqrt(double d) {
 // half-warps:  w = c[j] / d_j ;  c[s] -= w * a_sj  (s > j),  where a_sj = slot j of matrix lane s comes from ONE shuffle that
 // serves both halves (matrix lane r: a_rs -= (a_rj / d_j) a_sj;  inverse lane q: e_s[q] -= (a_sj / d_j) e_j[q]).
 // No shared-memory round trip, no __syncwarp, no per-element predicate.  The pivot chain is shuffle -> reciprocal (MUFU seed
-// + 2 Newton steps, ~47 cycles) -> multiply -> fma; the column shuffles are issued under the reciprocal (measured on B200:
-// a 64-bit shuffle issues every ~8.6 cycles, DFMA latency 8.4).  Square roots are taken once at the end, one per lane.
+// + 2 Newton steps) -> multiply -> fma; the column shuffles are issued under the reciprocal (tools/lat_microbench.cu
+// measures these latencies).  Square roots are taken once at the end, one per lane.
 // On exit:  lane r < N:   c[k] = L[r][k]      (k <= r; Cholesky factor, A = L L^T)
 //           lane 16 + q:  c[k] = (L^-1)[k][q] (k >= q; exactly 0 above the diagonal)
 //           rs (every lane l): 1 / L[l & 15][l & 15] on lanes with (l & 15) < N.

@@ -1,4 +1,4 @@
-// riccati_backward.cuh -- batched backward Riccati recursion, one CTA per OCP instance, sm_100a.
+// riccati_backward.cuh -- batched backward Riccati recursion, one CTA per OCP instance, sm_90a.
 //
 // Restates (as a different program) what the reference does in
 //   RiccatiRecursion::backwardRiccatiRecursion                 src/riccati/riccati_recursion.cpp:32-80
@@ -13,8 +13,8 @@
 //  * All dense contractions run on the fp64 tensor pipe (mma.sync m8n8k4): GEMM warp w owns the 8-row band w of every
 //    product; extents that are not multiples of 8 use one pulled-back (overlapping) tile instead of padding.
 //  * Warp specialisation: TX "GEMM warps" do A^T P, (A^T P) A, H; one extra "factor warp" builds
-//    G = Quu + Bv^T P_vv Bv, its Cholesky L and L^-1 concurrently (r1 profile: 53 % of all stall samples were warps
-//    parked at barriers behind a single-warp Cholesky + per-thread triangular solves).
+//    G = Quu + Bv^T P_vv Bv, its Cholesky L and L^-1 concurrently, so that the GEMM warps do not wait at barriers behind a
+//    single-warp Cholesky + per-thread triangular solves.
 //  * algebra: z = s+ - P+ Fx gives  lu' = lu - Bv^T z_v,  t1 = A^T z - lx;  with  Y = L^-1 H^T,  y = L^-1 lu':
 //        P = sym(F - Y^T Y),   s = t1 + Y^T y,   K = -L^-T Y,   k = -L^-T y
 //    so the critical path needs no triangular solve and no K; K, k are produced by the factor warp off the critical
@@ -572,7 +572,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
       }
     }
     RBT_TL(i, 7);
-    if (tid == 0) tma_store_wait_read();  // the previous stage's bulk store of P has long read shared memory (issued ~3 us ago)
+    if (tid == 0) tma_store_wait_read();  // the previous stage's bulk store of P has long read shared memory (issued a whole stage ago)
     __syncthreads();  // ---- barrier 2: AtP/H/t1 (GEMM warps) and G = L L^T, lu' (factor warp) are complete
     RBT_TL(i, 8);
 
@@ -862,7 +862,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
     // ================= P = F - Y^T Y.  Symmetric stages (no switching constraint, no factorized-KKT output): the accumulator
     // fragments with r <= c go straight to BOTH mirror positions of the next stage's P in shared memory (P+ is dead: its last
     // readers were the phase A / B products, two barriers ago), and P leaves for HBM as ONE bulk shared -> global copy after
-    // the barrier.  (The element-wise symmetrise-and-store loop this replaces was 16 % of the sweep's instructions.)
+    // the barrier, instead of an element-wise symmetrise-and-store loop.
     const bool fastP = symF && fct == nullptr;
     if (gemm_warp) {
       // rows the pulled-back last band shares with the band before it are stored by their owner only (identical values)

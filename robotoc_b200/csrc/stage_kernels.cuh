@@ -102,9 +102,8 @@ __device__ __noinline__ void se3_jac_inverse_dev(const double* Jac, double* Jinv
 // every lane with 16-byte loads.  Rows / columns >= n are carried as identity (no per-element predicates: entries above the
 // diagonal of a lane's row are scratch, and what is stored beyond n is the identity).  Pivots use the MUFU-seeded reciprocal
 // square root.  Writes L over A and dinv[j] = 1 / L[j][j].
-// (The first version predicated every update on the runtime n and on lane >= k and used the IEEE rsqrt: 2.8 k instructions for
-//  NMAX = 18 -- 52 % of mjtjinv_kernel's program; a pure shuffle version is 4.1 k: ptxas wraps every shuffle of this
-//  divergence-prone code in WARPSYNC / ENDCOLLECTIVE.)
+// (Predicating every update on the runtime n and on lane >= k costs many more instructions; a pure shuffle version is larger
+//  too: ptxas wraps every shuffle of this divergence-prone code in WARPSYNC / ENDCOLLECTIVE.)
 template <int NMAX, int LD>
 __device__ __forceinline__ bool warp_cholesky_ld(double* A, int n, double* dinv) {
   static_assert(NMAX <= 32 && NMAX % 2 == 0 && LD % 2 == 0, "one row per lane; 16-byte column loads of row pairs");
@@ -507,8 +506,8 @@ __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_C
     // Qqq += sum_c dg_dq^T diag(w) dg_dq          friction_cone.cpp:217-218  (box diagonal below)
     // One NV x (5 ncon) x NV product on the tensor pipe: the cone rows of all contacts are the contraction index k = 5 ci + r
     // (rows of inactive contacts were zeroed above).  Warp w < TV owns row band w (A fragment and its weight loaded once per
-    // k-step, TV column tiles); the other warps do the Qqf / Qff terms meanwhile.  (A tile-per-warp version with generic
-    // operand lambdas spent 33 instructions per DMMA: 12 % of this kernel's instructions for 45 DMMAs.)
+    // k-step, TV column tiles); the other warps do the Qqf / Qff terms meanwhile.  (Generic operand lambdas per tile would spend
+    // far more index arithmetic per DMMA.)
     constexpr int KC = 5 * (NFM / 3);
     static_assert(KC % 4 == 0 && TV < NTHR / 32, "cone rows fill whole k-steps; at least one warp left for Qqf / Qff");
     if (warp < TV) {
@@ -574,8 +573,8 @@ __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_C
       }
     }
     __syncthreads();  // the Qqq diagonal below touches elements the loop above also updates
-    // (measured: folding the diagonal weight into the tile epilogue to drop this barrier is 2.7 % SLOWER -- the divergent
-    //  gather costs more issue slots than the barrier wait it saves)
+    // (folding the diagonal weight into the tile epilogue would drop this barrier at the price of a divergent gather in
+    //  every tile)
     // gradients and diagonals, one target per thread spread over the warps
     if (warp == 0 && lane < NV) {
       double w, gs;
@@ -676,8 +675,8 @@ __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_C
   }
   __syncthreads();
   // R and the contact rows [Qaf | Quf] are final and only read from here on: they go to the expansion record as two bulk
-  // shared -> global copies that run under the Hessian condensing (the element-wise copy-out loops were 9 % of the kernel's
-  // instructions; the acceleration rows of Qafqv / Qafu are not stored at all -- rbt_stage_layout.h)
+  // shared -> global copies that run under the Hessian condensing (no element-wise copy-out loop; the acceleration rows of
+  // Qafqv / Qafu are not stored at all -- rbt_stage_layout.h)
   if (tid == 0) {
     tma_store_fence();
     tma_store_1d(ex + S.e_R, sR, uint32_t(NVF * NX) * 8u);
@@ -789,7 +788,6 @@ __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_C
   // ---- state equation rows                                 contact_dynamics.cpp:130-135, impact_dynamics.cpp:71-74
   const double sdt = impact ? 1.0 : dt;
   {  // thread = (pair of rows, column phase): 16-byte stores, the rows decide the formula once, no div / mod in the loop
-     // (the flat element loop was 13 % of the kernel's executed instructions, a row-per-thread version still 10 %)
     constexpr int RP = NX / 2, CP = NTHR / RP;  // row pairs ; columns written per pass
     static_assert(NX % 2 == 0 && NV % 2 == 0 && NVF % 2 == 0 && CP >= 1, "row pairs never straddle the q | v boundary");
     if (tid < CP * RP) {
@@ -869,8 +867,7 @@ __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_C
   }
   // ---- STO sensitivities + scaling                         contact_dynamics.cpp:156-163, intermediate_stage.cpp:140-148
   // Only grid points of a phase whose duration is optimised carry them: the sweeps read hx, hu, h, Qtt and haf under the
-  // same condition (riccati_backward.cuh: `if (sto)`, update_kernel: dts != 0), so the other grid points skip the work
-  // (6 % of this kernel's instructions on a schedule without switching-time optimisation).
+  // same condition (riccati_backward.cuh: `if (sto)`, update_kernel: dts != 0), so the other grid points skip the work.
   if (!impact && (c.sto || c.sto_next)) {
     const double g1 = 1.0 / c.ngrids_in_phase;
     matvec_T(sR, NVF, NVF, NX, vhaf, tid, NTHR, [&](int ii, double a) {
@@ -1126,7 +1123,7 @@ __device__ __forceinline__ void integrate_free_flyer_dev(double* q, const double
 }
 
 #ifndef RBT_UPD_MIN_CTAS
-#define RBT_UPD_MIN_CTAS 12  // latency-bound streaming kernel: 12 CTAs/SM (40 registers) is 25 % faster than 8 (63 registers); 14: slower
+#define RBT_UPD_MIN_CTAS 12  // latency-bound streaming kernel: many resident CTAs (12/SM at 40 registers) hide its load latency
 #endif
 template <int NV, int NU, int NFM>
 __global__ void __launch_bounds__(XTHR, RBT_UPD_MIN_CTAS) update_kernel(const StageParams p) {

@@ -1,5 +1,5 @@
 """Host-side mirror of the part of robotoc::DirectMultipleShooting that is on the hot path
-(/root/reference/include/robotoc/ocp/direct_multiple_shooting.hpp:86-199, src/ocp/direct_multiple_shooting.cpp):
+(robotoc/include/robotoc/ocp/direct_multiple_shooting.hpp:86-199, src/ocp/direct_multiple_shooting.cpp):
 
   evalKKT (its "Forms linear system" tail, :129-159 -> intermediate_stage.cpp:133-148)   -> condense()
   computeStepSizes :174-199, maxPrimalStepSize / maxDualStepSize :202-209                -> computeStepSizes(), max*StepSize()

@@ -1,4 +1,4 @@
-"""Grid types and the GridInfo mirror (/root/reference/include/robotoc/ocp/grid_info.hpp:14-92).
+"""Grid types and the GridInfo mirror (robotoc/include/robotoc/ocp/grid_info.hpp:14-92).
 
 A drop-in host receives GridInfo from robotoc's own TimeDiscretization and fills the rbt_stage_ctrl table from it
 (include/robotoc_b200/riccati_recursion.hpp does exactly that in C++); this module only holds the field mirror, the

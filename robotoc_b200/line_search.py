@@ -1,5 +1,5 @@
 """Host-side mirror of robotoc::LineSearch's filter method for a BATCH of OCPs
-(/root/reference/include/robotoc/line_search/line_search.hpp, src/line_search/line_search.cpp:58-86,
+(robotoc/include/robotoc/line_search/line_search.hpp, src/line_search/line_search.cpp:58-86,
 line_search_settings.hpp, line_search_filter.cpp) on top of the C ABI (rbt_line_search_*).
 
 The reference evaluates the trial step sizes alpha_max * 0.75^k one after the other; here all trials are generated in one launch

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's Riccati classes, calling the CUDA library through its C ABI.
 
-  RiccatiRecursion          <-> /root/reference/include/robotoc/riccati/riccati_recursion.hpp:26-119
-  UnconstrRiccatiRecursion  <-> /root/reference/include/robotoc/riccati/unconstr_riccati_recursion.hpp
+  RiccatiRecursion          <-> robotoc/include/robotoc/riccati/riccati_recursion.hpp:26-119
+  UnconstrRiccatiRecursion  <-> robotoc/include/robotoc/riccati/unconstr_riccati_recursion.hpp
 
 Same method names and argument meaning; the per-stage containers (KKTMatrix, KKTResidual, RiccatiFactorization,
 Direction, aligned_vector<LQRPolicy>) are the packed numpy arrays described by robotoc_b200.layout.Layout,

@@ -1,7 +1,7 @@
 """Multi-GPU sharding of the OCP batch (SURVEY.md 8e).
 
 OCP instances are independent (no coupling between batch elements anywhere in OCPSolver::updateSolution,
-/root/reference/src/solver/ocp_solver.cpp:111-145), so the batch is split into contiguous blocks, one per rank / GPU;
+robotoc/src/solver/ocp_solver.cpp:111-145), so the batch is split into contiguous blocks, one per rank / GPU;
 there is no data-path collective inside an iteration.  The only exchange is ONE all-gather of the Newton step
 (direction records) so that every rank sees the whole step (north_star: "a single NCCL all-gather of the converged
 step").  torch.distributed is plumbing: NCCL over NVLink on GPUs, gloo in the CPU tests.

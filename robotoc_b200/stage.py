@@ -2,9 +2,9 @@
 
 Mirrors, on the host side,
   the tail of IntermediateStage/ImpactStage/TerminalStage::evalKKT ("Forms linear system",
-      /root/reference/src/ocp/intermediate_stage.cpp:133-148, impact_stage.cpp:115-121, terminal_stage.cpp:102-106),
+      robotoc/src/ocp/intermediate_stage.cpp:133-148, impact_stage.cpp:115-121, terminal_stage.cpp:102-106),
   DirectMultipleShooting::computeStepSizes / maxPrimalStepSize / maxDualStepSize / integrateSolution
-      (/root/reference/src/ocp/direct_multiple_shooting.cpp:174-241).
+      (robotoc/src/ocp/direct_multiple_shooting.cpp:174-241).
 The records are described in include/rbt_stage_layout.h.
 """
 import ctypes

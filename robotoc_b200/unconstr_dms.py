@@ -1,5 +1,5 @@
 """Host-side mirror of the hot-path part of robotoc::UnconstrDirectMultipleShooting
-(/root/reference/src/unconstr/unconstr_direct_multiple_shooting.cpp:88-179) for fixed-base robots without contacts:
+(robotoc/src/unconstr/unconstr_direct_multiple_shooting.cpp:88-179) for fixed-base robots without contacts:
 
   evalKKT's condensing tail (unconstr_intermediate_stage.cpp:96-98)           -> condense()
   computeStepSizes :128-146, maxPrimalStepSize / maxDualStepSize :149-156     -> computeStepSizes(), max*StepSize()

@@ -5,7 +5,8 @@
 The reference itself (Eigen3 + Pinocchio C++) cannot be built or imported in this image, and its test-suite holds no
 golden vectors (SURVEY.md section 4), so these fixtures pin the ORACLE (regression) and give the GPU tests a
 size-independent, file-based target; the oracle in turn is pinned by the identity tests (test_oracle_kkt.py,
-test_oracle_condense.py).  Inputs are regenerated from the seeds below by the tests; only outputs are stored.
+test_oracle_condense.py).  Inputs are regenerated from the seeds below by the tests; only outputs are stored, each record
+array as a fixed, seeded sample of every section of every record (golden_sample.py).
 """
 import ctypes
 import os
@@ -24,6 +25,11 @@ from robotoc_b200 import ANYMAL, Layout, ULayout  # noqa: E402
 from robotoc_b200.stage import StageDims, StageLayout, anymal_constraint_table  # noqa: E402
 from synth import make_stage_inputs  # noqa: E402
 from synth import make_kkt, make_unconstr_kkt  # noqa: E402
+sys.path.insert(0, HERE)
+from golden_sample import groups, layout_bounds, put  # noqa: E402
+
+PATH = os.path.join(HERE, "golden_r1.npz")
+FRAC = 0.3  # share of the nonzero entries of every record section that is stored
 
 SEEDS = {"riccati": 101, "riccati_sto": 102, "unconstr": 103, "iteration": 104, "iteration_sto": 105, "unconstr_iteration": 106}
 
@@ -89,8 +95,22 @@ if __name__ == "__main__":
     kkt_c, steps, sol, con = iteration_case()
     kkt_cs, steps_s, sol_s, con_s = iteration_case(True)
     ukkt, usteps, usol, ucon = unconstr_iteration_case()
-    np.savez_compressed(os.path.join(HERE, "golden_r1.npz"), ric=ric, d=d, ric_sto=ric_s, d_sto=d_s, uric=uric, ud=ud,
-                        kkt_condensed=kkt_c, steps=steps, sol=sol, con=con,
-                        kkt_condensed_sto=kkt_cs, steps_sto=steps_s, sol_sto=sol_s, con_sto=con_s,
-                        ukkt_condensed=ukkt, usteps=usteps, usol=usol, ucon=ucon)
-    print("wrote", os.path.join(HERE, "golden_r1.npz"), os.path.getsize(os.path.join(HERE, "golden_r1.npz")) // 1024, "KiB")
+    lib = oracle_lib.load()
+    K, UL = Layout(ANYMAL, getter=lib.orc_layout_get), ULayout(7, getter=lib.orc_ulayout_get)
+    sd = StageDims(ANYMAL, nf_max=12, n_contacts=4, n_box=anymal_constraint_table().n_box)
+    S = StageLayout(sd, getter=lib.orc_stage_layout_get)
+    sections = {"ric": (K, "r_"), "d": (K, "d_"), "ric_sto": (K, "r_"), "d_sto": (K, "d_"), "uric": (UL, "r_"), "ud": (UL, "d_"),
+                "kkt_condensed": (K, "k_"), "sol": (S, "s_"), "con": (S, "c_"), "kkt_condensed_sto": (K, "k_"),
+                "sol_sto": (S, "s_"), "con_sto": (S, "c_"), "ukkt_condensed": (UL, "k_"), "usol": None, "ucon": None}
+    arrays = dict(ric=ric, d=d, ric_sto=ric_s, d_sto=d_s, uric=uric, ud=ud, kkt_condensed=kkt_c, steps=steps, sol=sol, con=con,
+                  kkt_condensed_sto=kkt_cs, steps_sto=steps_s, sol_sto=sol_s, con_sto=con_s, ukkt_condensed=ukkt,
+                  usteps=usteps, usol=usol, ucon=ucon)
+    out = {}
+    for n, (key, a) in enumerate(arrays.items()):
+        if key not in sections:  # step sizes: stored whole
+            out[key] = a
+            continue
+        sec = sections[key]
+        put(out, key, a, groups(a, layout_bounds(sec[0], sec[1], a.shape[-1]) if sec else None), 100 + n, frac=FRAC, k_min=3, k_z=1)
+    np.savez_compressed(PATH, **out)
+    print("wrote", PATH, os.path.getsize(PATH) // 1024, "KiB")

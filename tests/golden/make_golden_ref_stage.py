@@ -1,7 +1,9 @@
 """Generates tests/golden/golden_ref_stage_r2.npz: one FULL hot-path iteration computed by the reference's own code
-(tests/ref_lib.reference_iteration: /root/reference/src/dynamics, src/constraints, src/core and src/riccati compiled unmodified,
+(tests/ref_lib.reference_iteration: robotoc's src/dynamics, src/constraints, src/core and src/riccati compiled unmodified,
 oracle/Makefile.ref) on the small event schedule with switching-time optimisation (Intermediate, Lift, switching-constraint and
-Impact stages), batch 1.  Only runs where /root/reference exists:   python tests/golden/make_golden_ref_stage.py"""
+Impact stages), batch 1; a fixed, seeded sample of every section of every record (golden_sample.py), the performance
+index whole.  Only runs where a robotoc source tree exists:
+    ROBOTOC_REFERENCE=<robotoc source tree> python tests/golden/make_golden_ref_stage.py"""
 import os
 import sys
 
@@ -11,14 +13,29 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, HERE)
 
 from helpers import small_event_schedule  # noqa: E402
 from robotoc_b200 import ANYMAL  # noqa: E402
 from robotoc_b200.stage import StageDims, anymal_constraint_table  # noqa: E402
 from synth import make_stage_inputs  # noqa: E402
+from golden_sample import groups, layout_bounds, put  # noqa: E402
+
+PATH = os.path.join(HERE, "golden_ref_stage_r2.npz")
+FRAC = 0.3  # share of the nonzero entries of every record section that is stored
 
 SEED, BATCH = 301, 1
 KEYS = ("kkt", "cc_cond", "ric", "d", "cc_exp", "xd_exp", "steps", "d_upd", "xd_upd", "cc_upd", "ex_upd", "perf_stage")
+
+
+def stage_groups(a, key, S, K):
+    """Per-section groups of a stage-layer record of reference_iteration (sections of the layout the record follows)."""
+    prefix = {"kkt": "k_", "ric": "r_", "d": "d_", "d_upd": "d_", "cc_cond": "c_", "cc_exp": "c_", "cc_upd": "c_",
+              "xd_exp": "x_", "xd_upd": "x_", "ex_upd": "e_"}.get(key)
+    if prefix is None:
+        return groups(a)
+    lay = K if prefix in ("k_", "r_", "d_") else S
+    return groups(a, layout_bounds(lay, prefix, a.shape[-1]))
 
 
 def problem(S_getter=None, K_getter=None, impact_cones=False):
@@ -38,11 +55,14 @@ if __name__ == "__main__":
     import ref_lib
     lib = oracle_lib.load()
     table, sd, S, K, ctrl, lin, con, sol, dx0 = problem(lib.orc_stage_layout_get, lib.orc_layout_get)
-    out = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
-    data = {k: out[k] for k in KEYS}
-    table, sd, S, K, ctrl, lin, con, sol, dx0 = problem(lib.orc_stage_layout_get, lib.orc_layout_get, impact_cones=True)
-    out = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
-    data.update({"ic_" + k: out[k] for k in KEYS})
-    path = os.path.join(HERE, "golden_ref_stage_r2.npz")
-    np.savez_compressed(path, **data)
-    print("wrote", path, os.path.getsize(path) // 1024, "KiB")
+    data = {}
+    for pre, icone in (("", False), ("ic_", True)):
+        table, sd, S, K, ctrl, lin, con, sol, dx0 = problem(lib.orc_stage_layout_get, lib.orc_layout_get, impact_cones=icone)
+        out = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
+        for n, k in enumerate(KEYS):
+            if k in ("steps", "perf_stage"):
+                data[pre + k] = out[k]
+            else:
+                put(data, pre + k, out[k], stage_groups(out[k], k, S, K), SEED + n, frac=FRAC, k_min=3, k_z=1)
+    np.savez_compressed(PATH, **data)
+    print("wrote", PATH, os.path.getsize(PATH) // 1024, "KiB")

@@ -2,7 +2,7 @@
 with it.  Shared by the -m gpu parity tests, __graft_entry__.smoke() and the pre-timing check of bench.py.
 
   condense -> backward Riccati -> forward Riccati -> expand + step sizes -> update
-  (the linear-algebra body of OCPSolver::updateSolution, /root/reference/src/solver/ocp_solver.cpp:118-144)
+  (the linear-algebra body of OCPSolver::updateSolution, robotoc/src/solver/ocp_solver.cpp:118-144)
 """
 import ctypes
 

@@ -1,7 +1,7 @@
-"""ctypes wrapper around oracle/_ref/libref_riccati.so -- the REFERENCE's own Riccati sources (/root/reference/src/riccati,
+"""ctypes wrapper around oracle/_ref/libref_riccati.so -- the REFERENCE's own Riccati sources (robotoc's src/riccati,
 src/core), compiled unmodified against the Eigen / Robot stand-ins of oracle/shim (oracle/Makefile.ref).  TEST
-INFRASTRUCTURE: it pins the oracle.  The library can only be (re)built where /root/reference exists; a prebuilt copy travels
-with the tree (git-ignored, not gpurun-ignored)."""
+INFRASTRUCTURE: the generators under tests/golden/ use it to store what the reference computes.  The library can only be
+built where a robotoc source tree is available: set ROBOTOC_REFERENCE to it."""
 import ctypes
 import os
 import subprocess
@@ -11,17 +11,17 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_DIR = os.path.join(ROOT, "oracle")
 LIB = os.path.join(ORACLE_DIR, "_ref", "libref_riccati.so")
-REFERENCE = os.environ.get("ROBOTOC_REFERENCE", "/root/reference")
+REFERENCE = os.environ.get("ROBOTOC_REFERENCE", "")
 
 _lib = None
 
 
 def available():
-    return os.path.exists(LIB) or os.path.isdir(os.path.join(REFERENCE, "src", "riccati"))
+    return os.path.exists(LIB) or (bool(REFERENCE) and os.path.isdir(os.path.join(REFERENCE, "src", "riccati")))
 
 
 def build():
-    if os.path.isdir(os.path.join(REFERENCE, "src", "riccati")):
+    if REFERENCE and os.path.isdir(os.path.join(REFERENCE, "src", "riccati")):
         subprocess.run(["make", "-s", "-C", ORACLE_DIR, "-f", "Makefile.ref", f"REF={REFERENCE}"], check=True)
 
 

@@ -1,8 +1,8 @@
 """TEST FIXTURE (not product code): control-table producer for the BASELINE schedules.
 
 Restates robotoc::TimeDiscretization::discretize / correctTimeSteps
-(/root/reference/src/ocp/time_discretization.cpp:43-262) and the event bookkeeping of
-robotoc::ContactSequence (/root/reference/src/planner/contact_sequence.cpp:55-95) as far as the
+(robotoc/src/ocp/time_discretization.cpp:43-262) and the event bookkeeping of
+robotoc::ContactSequence (robotoc/src/planner/contact_sequence.cpp:55-95) as far as the
 kernels need it: the per-grid-point GridInfo (grid_info.hpp:25-92) and, from it, the rbt_stage_ctrl
 table shared by a batch of OCPs.  A real drop-in takes GridInfo from robotoc's own class.
 """
@@ -250,7 +250,7 @@ def stage_ctrl_array(td: TimeDiscretization, ev: ContactEvents):
 
 
 def anymal_trot_events() -> ContactEvents:
-    """Contact schedule of /root/reference/examples/anymal/trot.cpp:41-47,172-190 (cycle=1):
+    """Contact schedule of robotoc/examples/anymal/trot.cpp:41-47,172-190 (cycle=1):
     stand(12) -lift@0.04-> LF+RH(6) -impact@0.54-> stand -lift@0.58-> LH+RF(6) -impact@1.08-> stand; T=1.12."""
     # contact order LF, LH, RF, RH (trot.cpp:34-37)
     ev = ContactEvents(phase_dimf=[12], phase_mask=[0b1111])
@@ -263,7 +263,7 @@ def anymal_trot_events() -> ContactEvents:
 
 
 def anymal_jump_sto_events() -> ContactEvents:
-    """Contact schedule of /root/reference/examples/anymal/jump_sto.cpp:42-48,131-140:
+    """Contact schedule of robotoc/examples/anymal/jump_sto.cpp:42-48,131-140:
     stand(12) -lift@0.4 (sto)-> flying(0) -impact@0.9 (sto)-> stand; T=1.7."""
     ev = ContactEvents(phase_dimf=[12], phase_mask=[0b1111])
     ev.push_back(False, 0.70 - 0.3, 0, sto=True, post_mask=0)

@@ -1,9 +1,9 @@
 """TEST FIXTURE (not product code): synthetic, structure-faithful KKT / linearization inputs (there is no Pinocchio here to linearise a real robot).
 
 Recipes follow the reference's own test factories with FIXED seeds:
-  /root/reference/test/test_helper/kkt_factory.cpp:7-64        (CreateSplitKKTMatrix / Residual)
-  /root/reference/test/riccati/riccati_factorizer_test.cpp:131-140 (switching-constraint blocks)
-  /root/reference/test/riccati/unconstr_riccati_recursion_test.cpp:33-46 (unconstrained horizon)
+  robotoc/test/test_helper/kkt_factory.cpp:7-64        (CreateSplitKKTMatrix / Residual)
+  robotoc/test/riccati/riccati_factorizer_test.cpp:131-140 (switching-constraint blocks)
+  robotoc/test/riccati/unconstr_riccati_recursion_test.cpp:33-46 (unconstrained horizon)
 "Random" is U(-1,1) like Eigen::Random.  Documented deviation (SURVEY.md 8d): the velocity rows of Fxx are
 `Fvq = dt*R, Fvv = I + dt*R, Fvu = dt*R` and the floating-base 6x6 blocks are `I + dt*R` / `dt*(I+R)`, which is the
 structure condensing produces (contact_dynamics.cpp:130-134, state_equation.cpp:80-82) and keeps a 40-90 step

@@ -1,9 +1,8 @@
-"""The reference's own outputs (tests/golden/golden_ref_r2.npz, made by tests/golden/make_golden_ref.py from
-/root/reference/src/riccati compiled unmodified) as the pin:
-  CPU:  the oracle (oracle/riccati_oracle.c) reproduces them -- this is what makes the oracle a trustworthy checker on the
-        GPU box, where /root/reference does not exist;
-  CPU:  where oracle/_ref can be built or has travelled, the oracle is also compared with the live reference library on
-        further seeds, every field of every record;
+"""The reference's own outputs (tests/golden/golden_ref_r2.npz, a seeded sample of every record section, made by tests/golden/make_golden_ref.py from robotoc's
+src/riccati compiled unmodified) as the pin:
+  CPU:  the oracle (oracle/riccati_oracle.c) reproduces them -- this is what makes the oracle a trustworthy checker;
+  CPU:  the oracle equals the reference code on further seeds, every field of every record, on a fixed sample of entries
+        (tests/golden/golden_ref_live.npz, made by tests/golden/make_golden_ref_live.py);
   GPU:  the CUDA path reproduces them through the C ABI."""
 import os
 import sys
@@ -14,11 +13,13 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_ref as mg  # noqa: E402
+from golden_sample import load, restore  # noqa: E402
+import make_golden_ref_live as mgl  # noqa: E402
 
 import oracle_lib  # noqa: E402
 from robotoc_b200 import ANYMAL, Layout, ULayout  # noqa: E402
 
-G = np.load(os.path.join(HERE, "golden", "golden_ref_r2.npz"))
+G = load(mg.PATH)
 TOL = 1e-10  # relative to the array's scale; measured agreement oracle <-> reference code: 1e-15 .. 3e-15
 
 
@@ -34,8 +35,8 @@ def test_oracle_reproduces_reference_golden(name):
     kk, ric, d, info = oracle_lib.riccati_batch(ANYMAL, L, ctrl, kkt, dx0)
     assert info == 0
     got = ric if full else mg.trim(L, ric)
-    assert _rel(got, G[name + "_ric"]) < TOL
-    assert _rel(d, G[name + "_dir"]) < TOL
+    assert _rel(got, restore(G, name + "_ric", got)) < TOL
+    assert _rel(d, restore(G, name + "_dir", d)) < TOL
 
 
 def test_oracle_reproduces_reference_golden_unconstr():
@@ -45,20 +46,15 @@ def test_oracle_reproduces_reference_golden_unconstr():
     u = mg.UNCONSTR
     kk, ric, d, info = oracle_lib.unconstr_batch(7, UL, u["N"], u["dt"], kkt, dx0)
     assert info == 0
-    assert _rel(ric, G["unconstr_ric"]) < TOL and _rel(d, G["unconstr_dir"]) < TOL
+    assert _rel(ric, restore(G, "unconstr_ric", ric)) < TOL and _rel(d, restore(G, "unconstr_dir", d)) < TOL
 
 
-def _ref_or_skip():
-    import ref_lib
-    if not ref_lib.available():
-        pytest.skip("oracle/_ref not built and /root/reference not present")
-    return ref_lib
+GL = load(mgl.PATH)
 
 
-@pytest.mark.parametrize("name,seed", [("small", 31), ("small_sto", 32), ("trot_n40", 33), ("jump_sto_n80", 34)])
+@pytest.mark.parametrize("name,seed", mgl.RICCATI_CASES)
 def test_oracle_equals_live_reference_every_field(name, seed):
     """Every field of every Riccati / direction record and the mutated KKT blocks (F, H, G, lu'), batch 3, fresh seeds."""
-    ref_lib = _ref_or_skip()
     from synth import make_kkt
     lib = oracle_lib.load()
     L = Layout(ANYMAL, getter=lib.orc_layout_get)
@@ -66,9 +62,8 @@ def test_oracle_equals_live_reference_every_field(name, seed):
     kkt, dx0 = make_kkt(ANYMAL, L, ctrl, batch=3, seed=seed)
     kk_o, ric_o, d_o, info = oracle_lib.riccati_batch(ANYMAL, L, ctrl, kkt, dx0)
     assert info == 0
-    kk_r, ric_r, d_r = ref_lib.riccati_batch(ANYMAL, L, ctrl, kkt, dx0)
-    fields = sorted((getattr(L, f), f) for f in ("r_P r_s r_K r_k r_M r_m r_Psi r_Phi r_T r_W r_psix r_psiu r_phix r_phiu r_mt "
-                                                  "r_mtn r_sc r_dtsdx r_stosc").split())
+    kk_r, ric_r, d_r = (restore(GL, f"ric_{name}_{k}", a) for k, a in (("kkt", kk_o), ("ric", ric_o), ("dir", d_o)))
+    fields = sorted((getattr(L, f), f) for f in mgl.RIC_FIELDS)
     ends = [o for o, _ in fields[1:]] + [L.r_stosc + 2]
     for (o, f), e in zip(fields, ends):
         a, b = ric_o[..., o:e], ric_r[..., o:e]
@@ -85,14 +80,13 @@ def test_oracle_equals_live_reference_every_field(name, seed):
 
 
 def test_oracle_equals_live_reference_unconstr():
-    ref_lib = _ref_or_skip()
     from synth import make_unconstr_kkt
     lib = oracle_lib.load()
     UL = ULayout(7, getter=lib.orc_ulayout_get)
-    for N, dt, seed in ((20, 0.05, 41), (50, 0.02, 42)):
+    for N, dt, seed in mgl.UNCONSTR_CASES:
         kkt, dx0 = make_unconstr_kkt(7, UL, N, 3, seed)
         kk_o, ric_o, d_o, info = oracle_lib.unconstr_batch(7, UL, N, dt, kkt, dx0)
-        kk_r, ric_r, d_r = ref_lib.unconstr_batch(7, UL, N, dt, kkt, dx0)
+        kk_r, ric_r, d_r = (restore(GL, f"unconstr_{N}_{k}", a) for k, a in (("kkt", kk_o), ("ric", ric_o), ("dir", d_o)))
         assert info == 0 and _rel(ric_o, ric_r) < TOL and _rel(d_o, d_r) < TOL and _rel(kk_o, kk_r) < TOL
 
 
@@ -108,7 +102,7 @@ def test_cuda_reproduces_reference_golden(name):
     rr.forwardRiccatiRecursion(dx0)
     assert int(rr.info().max()) == 0
     ric, d = rr.getRiccatiFactorization(), rr.getDirection()
-    ref_ric = G[name + "_ric"]
+    ref_ric = restore(G, name + "_ric", ric if full else mg.trim(L, ric))
     if full:
         # stage-conditional sections the reference leaves at their constructor zeros are zero here too; W at ns == nu is noise
         got = ric
@@ -118,7 +112,7 @@ def test_cuda_reproduces_reference_golden(name):
         assert _rel(got, ref_ric) < 1e-8
     else:
         assert _rel(mg.trim(L, ric), ref_ric) < 1e-8
-    assert _rel(d, G[name + "_dir"]) < 1e-8
+    assert _rel(d, restore(G, name + "_dir", d)) < 1e-8
     rr.close()
 
 
@@ -132,6 +126,7 @@ def test_cuda_reproduces_reference_golden_unconstr():
     ur.backwardRiccatiRecursion(kkt)
     ur.forwardRiccatiRecursion(dx0)
     assert int(ur.info().max()) == 0
-    assert _rel(ur.getRiccatiFactorization(), G["unconstr_ric"]) < 1e-8
-    assert _rel(ur.getDirection(), G["unconstr_dir"]) < 1e-8
+    ric, d = ur.getRiccatiFactorization(), ur.getDirection()
+    assert _rel(ric, restore(G, "unconstr_ric", ric)) < 1e-8
+    assert _rel(d, restore(G, "unconstr_dir", d)) < 1e-8
     ur.close()

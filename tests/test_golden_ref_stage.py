@@ -1,8 +1,8 @@
 """The stage layer (condensing, expansion, step sizes, slack / dual update: SURVEY.md 8a rows a10-a16) pinned against the
-reference's own code.  tests/golden/golden_ref_stage_r2.npz holds one full iteration computed by /root/reference's sources
+reference's own code.  tests/golden/golden_ref_stage_r2.npz holds (a seeded sample of) one full iteration computed by robotoc's sources
 (make_golden_ref_stage.py);
-  CPU: the oracle reproduces it; where oracle/_ref is available the oracle is also compared with the live reference code on the
-       BASELINE trot schedule and further seeds;
+  CPU: the oracle reproduces it; it is also compared with the reference code on the BASELINE trot schedule and further seeds
+       (a fixed sample of every record: tests/golden/golden_ref_live.npz, make_golden_ref_live.py);
   GPU: the CUDA path reproduces it through the C ABI."""
 import os
 import sys
@@ -13,12 +13,20 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_ref_stage as mg  # noqa: E402
+from golden_sample import load, restore  # noqa: E402
+import make_golden_ref_live as mgl  # noqa: E402
 
 import oracle_lib  # noqa: E402
 from iteration_check import mask_unread_sto, oracle_iteration, reference_view_of_expansion  # noqa: E402
 from robotoc_b200.grid import IMPACT, TERMINAL  # noqa: E402
 
-G = np.load(os.path.join(HERE, "golden", "golden_ref_stage_r2.npz"))
+G = load(mg.PATH)
+
+
+def _golden(got, impact_cones):
+    """The stored reference iteration (a seeded sample of every record section), put into copies of the records under test."""
+    pre = "ic_" if impact_cones else ""
+    return {k: restore(G, pre + k, got[k]) for k in mg.KEYS if k in got}
 TOL = 1e-10
 
 
@@ -76,9 +84,10 @@ def test_oracle_reproduces_the_reference_iteration_golden(impact_cones):
     lib = oracle_lib.load()
     table, sd, S, K, ctrl, lin, con, sol, dx0 = mg.problem(lib.orc_stage_layout_get, lib.orc_layout_get, impact_cones)
     got = oracle_iteration(sd, S, K, table, ctrl, lin, con, sol, dx0)
-    ref = {k[3:]: G[k] for k in G.files if k.startswith("ic_")} if impact_cones else G
+    ref = _golden(got, impact_cones)
     if impact_cones:  # the impact cones must matter: the iteration differs from the one without them
-        assert np.max(np.abs(ref["ric"] - G["ric"])) > 1e-6 and abs(float(ref["steps"][0, 0]) - float(G["steps"][0, 0])) >= 0.0
+        both, a, b = np.intersect1d(G["ic_ric#i"], G["ric#i"], return_indices=True)
+        assert np.max(np.abs(G["ic_ric#v"][a] - G["ric#v"][b])) > 1e-6
     _cmp_records(S, K, ctrl, got, ref, TOL, impact_cones=impact_cones)
 
 
@@ -101,48 +110,25 @@ def _oracle_perf_stage(lib, sd, S, table, ctrl, lin, con):
 def test_oracle_performance_index_equals_the_reference_evalKKT_summary(impact_cones):
     """PerformanceIndex of every grid point (log barrier, primal / dual feasibility, squared KKT error) as the reference's own
     members compute it before condensing (OCPData / SplitKKTResidual / ConstraintsData / ContactDynamicsData ::KKTError etc.,
-    intermediate_stage.cpp:124-132, impact_stage.cpp:104-113, terminal_stage.cpp:94-100) -- golden fixture, and live where
-    oracle/_ref is available."""
+    intermediate_stage.cpp:124-132, impact_stage.cpp:104-113, terminal_stage.cpp:94-100) -- golden fixtures."""
     lib = oracle_lib.load()
     table, sd, S, K, ctrl, lin, con, sol, dx0 = mg.problem(lib.orc_stage_layout_get, lib.orc_layout_get, impact_cones)
     got = _oracle_perf_stage(lib, sd, S, table, ctrl, lin, con)
     ref = G["ic_perf_stage" if impact_cones else "perf_stage"]
     np.testing.assert_allclose(got, ref, rtol=1e-12, atol=1e-300)
     assert (ref[:, :, 3] > 0).all() and (ref[:, :-1, 0] != 0).any()
-    import ref_lib
-    if ref_lib.available():
-        from helpers import trot_schedule
-        from robotoc_b200 import ANYMAL, Layout, StageDims, StageLayout, anymal_constraint_table
-        from synth import make_stage_inputs
-        table = anymal_constraint_table(impact_friction_cone=impact_cones)
-        td, ev, ctrl = trot_schedule(40)
-        lin, con, sol, dx0 = make_stage_inputs(sd, S, ctrl, 1, 316, impact_cones=impact_cones)
-        rng = np.random.default_rng(5)
-        for i, c in enumerate(ctrl):  # give the switching-constraint residual something to measure
-            if c.ns > 0:
-                lin[:, i, S.l_p:S.l_p + c.ns] = rng.uniform(-1, 1, size=(1, c.ns))
-        live = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)["perf_stage"]
-        np.testing.assert_allclose(_oracle_perf_stage(lib, sd, S, table, ctrl, lin, con), live, rtol=1e-12, atol=1e-300)
+    table, ctrl, lin, con, dx0 = mgl.perf_case(sd, S, impact_cones)
+    np.testing.assert_allclose(_oracle_perf_stage(lib, sd, S, table, ctrl, lin, con), load(mgl.PATH)[f"perf_icone{int(impact_cones)}"],
+                               rtol=1e-12, atol=1e-300)
 
 
-@pytest.mark.parametrize("which,seed", [("small", 311), ("small_sto", 312), ("trot", 313), ("small_icone", 314), ("small_sto_icone", 315)])
+@pytest.mark.parametrize("which,seed", mgl.STAGE_CASES)
 def test_oracle_equals_live_reference_stage_layer(which, seed):
-    import ref_lib
-    if not ref_lib.available():
-        pytest.skip("oracle/_ref not built and /root/reference not present")
-    from helpers import small_event_schedule, trot_schedule
-    from robotoc_b200 import ANYMAL, Layout, StageDims, StageLayout, anymal_constraint_table
-    from synth import make_stage_inputs
     lib = oracle_lib.load()
-    icone = which.endswith("_icone")
-    table = anymal_constraint_table(impact_friction_cone=icone)
-    sd = StageDims(ANYMAL, nf_max=12, n_contacts=table.n_contacts, n_box=table.n_box)
-    S, K = StageLayout(sd, getter=lib.orc_stage_layout_get), Layout(ANYMAL, getter=lib.orc_layout_get)
-    td, ev, ctrl = {"small": small_event_schedule(False), "small_sto": small_event_schedule(True), "trot": trot_schedule(40),
-                    "small_icone": small_event_schedule(False), "small_sto_icone": small_event_schedule(True)}[which]
-    lin, con, sol, dx0 = make_stage_inputs(sd, S, ctrl, 1, seed, impact_cones=icone)
-    ref = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
+    table, sd, S, K, ctrl, lin, con, sol, dx0, icone = mgl.stage_case(which, seed, lib.orc_stage_layout_get, lib.orc_layout_get)
     got = oracle_iteration(sd, S, K, table, ctrl, lin, con, sol, dx0)
+    GL = load(mgl.PATH)
+    ref = {k: restore(GL, f"stage_{which}_{k}", got[k]) for k in mgl.STAGE_KEYS}
     _cmp_records(S, K, ctrl, got, ref, TOL, impact_cones=icone)
 
 
@@ -171,6 +157,5 @@ def test_cuda_reproduces_the_reference_iteration_golden(impact_cones):
     dms.integrateSolution(sol)
     got["d_upd"], got["xd_upd"], got["cc_upd"], got["ex_upd"] = (rr.getDirection(), dms.getExpandedDirection(), dms.getConstraintData(),
                                                                  reference_view_of_expansion(S, dms.getExpansionData()))
-    ref = {k[3:]: G[k] for k in G.files if k.startswith("ic_")} if impact_cones else G
-    _cmp_records(S, K, ctrl, got, ref, 1e-8, impact_cones=impact_cones)
+    _cmp_records(S, K, ctrl, got, _golden(got, impact_cones), 1e-8, impact_cones=impact_cones)
     rr.close()

@@ -68,7 +68,7 @@ def test_cpp_allgather_test_compiles_and_links(tmp_path):
 @pytest.mark.gpu
 def test_cpp_allgather_step_two_ranks(tmp_path):
     """Two ranks in one process (ncclCommInitAll) gather the packed Newton step through rbt_allgather_step.
-    Needs two GPUs: skipped (exit code 77) on a single-GPU box; run under `gpurun --gpus 2`."""
+    Needs two GPUs: skipped (exit code 77) on a single-GPU machine."""
     exe = _build_allgather(str(tmp_path))
     out = subprocess.run([exe], capture_output=True, text=True, timeout=180)
     print(out.stdout, out.stderr)

@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     L = _lib.lib()
     for name in declared:
         assert hasattr(L, name), name
-    assert b"sm_100a" in L.rbt_version()
+    assert b"sm_90a" in L.rbt_version()
 
 
 def test_no_cpu_fallback_without_device():

@@ -1,4 +1,4 @@
-"""Backward-sweep time vs CTAs resident per SM: batch = 148*k OCPs (one full wave of k CTAs/SM), k = 1..4.
+"""Backward-sweep time vs CTAs resident per SM: batch = (SM count)*k OCPs (one full wave of k CTAs/SM), k = 1..4.
 Tells whether the kernel is latency-bound (time flat in k) or throughput-bound (time ~ k)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-// Microbenchmark: FP64 DFMA vs DMMA (mma.sync.m8n8k4.f64) throughput on sm_100a.
+// Microbenchmark: FP64 DFMA vs DMMA (mma.sync.m8n8k4.f64) throughput on sm_90a.
 // Decides whether the Riccati GEMMs use tensor-pipe DMMA or CUDA-core DFMA.
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -53,11 +53,11 @@ __global__ void dfma_smem_kernel(double* out, int iters) {
 int main() {
   cudaDeviceProp p; cudaGetDeviceProperties(&p, 0);
   printf("device %s sms=%d clock=%d kHz\n", p.name, p.multiProcessorCount, p.clockRate);
-  double* out; cudaMalloc(&out, sizeof(double) * 148 * 64 * 1024);
+  double* out; cudaMalloc(&out, sizeof(double) * 132 * 64 * 1024);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   float ms;
   for (int threads : {128, 256, 512, 1024}) {
-    int blocks = 148 * (2048 / threads);
+    int blocks = 132 * (2048 / threads);
     int iters = 20000;
     dfma_kernel<<<blocks, threads>>>(out, 100, 1.0000001, 1e-9);
     cudaDeviceSynchronize();
@@ -75,7 +75,7 @@ int main() {
   }
   for (int threads : {160, 288}) {
     for (int bps : {1, 2, 4, 6}) {
-      int blocks = 148 * bps; int iters = 2000;
+      int blocks = 132 * bps; int iters = 2000;
       dfma_smem_kernel<<<blocks, threads>>>(out, 10);
       cudaDeviceSynchronize();
       cudaEventRecord(e0); dfma_smem_kernel<<<blocks, threads>>>(out, iters); cudaEventRecord(e1);

@@ -1,4 +1,4 @@
-// Single-warp dependent-chain latencies on sm_100a (cycles per op): DFMA, DMUL->DFMA, SHFL(64-bit)->DFMA, MUFU.RCP64H+2 Newton,
+// Single-warp dependent-chain latencies on sm_90a (cycles per op): DFMA, DMUL->DFMA, SHFL(64-bit)->DFMA, MUFU.RCP64H+2 Newton,
 // DMMA m8n8k4 accumulate chain, 5 independent DMMA accumulators, LDS->DFMA, and issue throughput of independent SHFL / DFMA.
 #include <cstdio>
 #include <cuda_runtime.h>
