@@ -189,6 +189,7 @@ int rbt_create(const rbt_dims* dims, int n_grid_max, int batch, int device, rbt_
     RBT_CUDA(h, cudaMalloc(&h->d_timeline, size_t(n_grid_max) * 32 * sizeof(long long)));
     RBT_CUDA(h, cudaMemset(h->d_timeline, 0, size_t(n_grid_max) * 32 * sizeof(long long)));
   }
+  RBT_CUDA(h, cudaMemset(h->d_kkt, 0, per * h->L.k_stride * 8));  // condensing skips the switching rows a stage lacks: keep them defined
   RBT_CUDA(h, cudaMemset(h->d_ric, 0, per * h->L.r_stride * 8));
   RBT_CUDA(h, cudaMemset(h->d_fact, 0, per * h->L.f_stride * 8));
   RBT_CUDA(h, cudaMemset(h->d_dir, 0, per * h->L.d_stride * 8));

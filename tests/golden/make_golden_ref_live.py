@@ -1,8 +1,11 @@
-"""Generates tests/golden/golden_ref_live.npz: the reference's own outputs (oracle/_ref/libref_riccati.so, the robotoc sources
-compiled unmodified by oracle/Makefile.ref) for the cases on which tests/ compare the oracle with the reference code, so that
+"""Generates tests/golden/golden_ref_live.npz and tests/golden/golden_ref_gaits.npz: the reference's own outputs
+(oracle/_ref/libref_riccati.so, the robotoc sources compiled unmodified by oracle/Makefile.ref) for the cases on which tests/ compare the oracle with the reference code, so that
 those comparisons run everywhere without a robotoc checkout.  Only runs where one exists:
 
-    ROBOTOC_REFERENCE=<robotoc source tree> python tests/golden/make_golden_ref_live.py
+    ROBOTOC_REFERENCE=<robotoc source tree> python tests/golden/make_golden_ref_live.py [live] [gaits]
+
+golden_ref_gaits.npz holds the cases on the crawl and contact-mask-walk schedules (odd contact counts, single-foot impacts,
+every contact mask); golden_ref_live.npz everything else.  Without arguments both files are written.
 
 Large records are stored as a fixed, seeded sample of every section of every record (golden_sample.py); small outputs are
 stored whole.
@@ -20,21 +23,38 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, HERE)
 
 from golden_sample import groups, layout_bounds, load, put, restore  # noqa: E402,F401  (load, restore: used by the tests)
-from helpers import small_event_schedule, trot_schedule  # noqa: E402
+from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, small_event_schedule, trot_schedule  # noqa: E402,E501
 
 PATH = os.path.join(HERE, "golden_ref_live.npz")
+GAITS_PATH = os.path.join(HERE, "golden_ref_gaits.npz")
 RIC_FIELDS = "r_P r_s r_K r_k r_M r_m r_Psi r_Phi r_T r_W r_psix r_psiu r_phix r_phiu r_mt r_mtn r_sc r_dtsdx r_stosc".split()
 STAGE_KEYS = ("kkt", "cc_cond", "ric", "d", "cc_exp", "xd_exp", "steps", "d_upd", "xd_upd", "cc_upd", "ex_upd")
 
 
 # ---- the cases (inputs are regenerated from these seeds by the tests)
-RICCATI_CASES = [("small", 31), ("small_sto", 32), ("trot_n40", 33), ("jump_sto_n80", 34)]
+RICCATI_CASES = [("small", 31), ("small_sto", 32), ("trot_n40", 33), ("jump_sto_n80", 34), ("crawl", 35), ("crawl_sto", 36)]
 UNCONSTR_CASES = [(20, 0.05, 41), (50, 0.02, 42)]
-STAGE_CASES = [("small", 311), ("small_sto", 312), ("trot", 313), ("small_icone", 314), ("small_sto_icone", 315)]
+STAGE_CASES = [("small", 311), ("small_sto", 312), ("trot", 313), ("small_icone", 314), ("small_sto_icone", 315), ("crawl", 317),
+               ("crawl_sto", 318), ("crawl_icone", 319), ("mask_walk", 320)]
+GAIT_CASES = ("crawl", "crawl_sto", "crawl_icone", "mask_walk")
 JOINT_LIMIT_CASES = ["small_sto", "trot"]
 
 
 JL_SCHEDULES = {"small_sto": lambda: small_event_schedule(True), "trot": lambda: trot_schedule(40)}
+SCHEDULES = {"small": lambda: small_event_schedule(False), "small_sto": lambda: small_event_schedule(True),
+             "trot": lambda: trot_schedule(40), "trot_n40": lambda: trot_schedule(40), "jump_sto_n80": lambda: jump_sto_schedule(80),
+             "crawl": lambda: crawl_schedule(54), "crawl_sto": lambda: crawl_schedule(54, sto=True),
+             "mask_walk": contact_mask_walk_schedule}
+
+
+def schedule(case):
+    """(TimeDiscretization, ContactEvents, control table) of a case; `<schedule>_icone` is `<schedule>` with impact cones."""
+    return SCHEDULES[case[:-len("_icone")] if case.endswith("_icone") else case]()
+
+
+def fixture_path(case):
+    """The fixture file that holds the reference's outputs of a case."""
+    return GAITS_PATH if case in GAIT_CASES else PATH
 
 
 def joint_limit_problem(sched, batch, seed):
@@ -65,8 +85,7 @@ def stage_case(which, seed, S_getter, K_getter):
     table = anymal_constraint_table(impact_friction_cone=icone)
     sd = StageDims(ANYMAL, nf_max=12, n_contacts=table.n_contacts, n_box=table.n_box)
     S, K = StageLayout(sd, getter=S_getter), Layout(ANYMAL, getter=K_getter)
-    td, ev, ctrl = {"small": small_event_schedule(False), "small_sto": small_event_schedule(True), "trot": trot_schedule(40),
-                    "small_icone": small_event_schedule(False), "small_sto_icone": small_event_schedule(True)}[which]
+    td, ev, ctrl = schedule(which)
     lin, con, sol, dx0 = make_stage_inputs(sd, S, ctrl, 1, seed, impact_cones=icone)
     return table, sd, S, K, ctrl, lin, con, sol, dx0, icone
 
@@ -95,25 +114,27 @@ def filter_rounds(case_rng):
     return amax, cost, viol, cost[:, 0] + 0.1, viol[:, 0] + 0.01
 
 
-def main():
+def main(outputs=("live", "gaits")):
     import oracle_lib
     import ref_lib
     import make_golden_ref_stage as mgs
     from robotoc_b200 import ANYMAL, Layout, ULayout
     from synth import make_kkt, make_unconstr_kkt
-    import make_golden_ref as mg
     assert ref_lib.available(), "set ROBOTOC_REFERENCE to a robotoc source tree"
     lib = oracle_lib.load()
     P = oracle_lib.ptr
-    out = {}
+    files = {PATH: {}, GAITS_PATH: {}}
+    out = files[PATH]
     L = Layout(ANYMAL, getter=lib.orc_layout_get)
     for name, seed in RICCATI_CASES:
-        td, ev, ctrl = mg.CASES[name][0]()
+        td, ev, ctrl = schedule(name)
         kkt, dx0 = make_kkt(ANYMAL, L, ctrl, batch=3, seed=seed)
         kk, ric, d = ref_lib.riccati_batch(ANYMAL, L, ctrl, kkt, dx0)
+        out = files[fixture_path(name)]
         put(out, f"ric_{name}_ric", ric, groups(ric, layout_bounds(L, "r_", L.r_stride)), seed, k_min=3, k_z=1)
         put(out, f"ric_{name}_dir", d, groups(d, layout_bounds(L, "d_", L.d_stride)), seed + 1, k_min=3, k_z=1)
         put(out, f"ric_{name}_kkt", kk, groups(kk, layout_bounds(L, "k_", L.k_stride)), seed + 2, k_min=3, k_z=1)
+    out = files[PATH]
     UL = ULayout(7, getter=lib.orc_ulayout_get)
     for N, dt, seed in UNCONSTR_CASES:
         kkt, dx0 = make_unconstr_kkt(7, UL, N, 3, seed)
@@ -121,11 +142,11 @@ def main():
         put(out, f"unconstr_{N}_ric", ric, groups(ric, layout_bounds(UL, "r_", UL.r_stride)), seed, k_min=3, k_z=1)
         put(out, f"unconstr_{N}_dir", d, groups(d, layout_bounds(UL, "d_", UL.d_stride)), seed + 1, k_min=3, k_z=1)
         put(out, f"unconstr_{N}_kkt", kk, groups(kk, layout_bounds(UL, "k_", UL.k_stride)), seed + 2, k_min=3, k_z=1)
-    for which, seed in STAGE_CASES:
-        table, sd, S, K, ctrl, lin, con, sol, dx0, icone = stage_case(which, seed, lib.orc_stage_layout_get, lib.orc_layout_get)
+    for case, seed in STAGE_CASES:
+        table, sd, S, K, ctrl, lin, con, sol, dx0, icone = stage_case(case, seed, lib.orc_stage_layout_get, lib.orc_layout_get)
         ref = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
         for k in STAGE_KEYS:
-            put(out, f"stage_{which}_{k}", ref[k], mgs.stage_groups(ref[k], k, S, K), seed, k_min=3, k_z=1)
+            put(files[fixture_path(case)], f"stage_{case}_{k}", ref[k], mgs.stage_groups(ref[k], k, S, K), seed, k_min=3, k_z=1)
     for icone in (False, True):
         table, sd, S, K, ctrl, lin, con, sol, dx0 = mgs.problem(lib.orc_stage_layout_get, lib.orc_layout_get, icone)
         table, ctrl, lin, con, dx0 = perf_case(sd, S, icone)
@@ -157,9 +178,11 @@ def main():
         # every entry the linearisation changes (group 0), plus a sample of the others (group 1)
         put(out, f"jl_{which}_lin", l_r, np.where(l_r != lin, 0, 1), 7, frac=(1.0, 0.0), k_min=(0, 256), k_z=(l_r.size, 32))
         put(out, f"jl_{which}_con", c_r, np.where(c_r != con, 0, 1), 8, frac=(1.0, 0.0), k_min=(0, 256), k_z=(c_r.size, 32))
-    np.savez_compressed(PATH, **out)
-    print("wrote", PATH, os.path.getsize(PATH) // 1024, "KiB;", ref.ref_version().decode())
+    for path, data in files.items():
+        if {PATH: "live", GAITS_PATH: "gaits"}[path] in outputs:
+            np.savez_compressed(path, **data)
+            print("wrote", path, os.path.getsize(path) // 1024, "KiB;", ref.ref_version().decode())
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:] or ("live", "gaits"))

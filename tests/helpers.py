@@ -4,7 +4,7 @@ import numpy as np
 from robotoc_b200 import ANYMAL, Layout
 from robotoc_b200.grid import IMPACT, LIFT, TERMINAL
 from schedule_fixture import (ContactEvents, TimeDiscretization, stage_ctrl_array, anymal_trot_events,
-                              anymal_jump_sto_events)
+                              anymal_jump_sto_events, anymal_crawl_events, contact_mask_walk_events)
 from synth import make_kkt, mat
 
 
@@ -27,6 +27,44 @@ def jump_sto_schedule(N=80):
     ev = anymal_jump_sto_events()
     td = TimeDiscretization(1.7, N).discretize(ev, 0.0, sto=True)
     return td, ev, stage_ctrl_array(td, ev)
+
+
+def crawl_schedule(N=54, sto=False):
+    """ANYmal crawl (anymal_crawl_events), T=2.16: three-foot stances, single-foot impacts (nf 3, ns 3) and two impacts at
+    which another foot lifts; with `sto` every event's switching time is optimised."""
+    ev = anymal_crawl_events(sto)
+    td = TimeDiscretization(2.16, N).discretize(ev, 0.0, sto=sto)
+    ctrl = stage_ctrl_array(td, ev)
+    types = [c.type for c in ctrl]
+    assert types.count(IMPACT) == 4 and types.count(LIFT) == 2 and types[-1] == TERMINAL
+    assert {c.nf for c in ctrl[:-1]} == {3, 9, 12} and {c.ns for c in ctrl} == {0, 3}
+    assert {c.contact_mask for c in ctrl if c.type == IMPACT} == {0b0001, 0b0010, 0b0100, 0b1000}
+    assert sum(1 for i, c in enumerate(ctrl) if c.type == IMPACT and ctrl[i - 1].contact_mask & ~ctrl[i + 1].contact_mask) == 2
+    assert all(c.sto for c in ctrl[:-1]) if sto else not any(c.sto or c.sto_next for c in ctrl)
+    return td, ev, ctrl
+
+
+# contact sets of contact_mask_walk_schedule's phases: all 16, impacts of 1 / 2 / 3 / 4 feet, impacts that also lift a foot
+MASK_WALK = [0b1111, 0b1110, 0b1100, 0b1000, 0b0000, 0b0101, 0b0001, 0b1011, 0b0011, 0b0010, 0b0110, 0b0100, 0b1101, 0b1001,
+             0b1010, 0b0111, 0b1111, 0b0000, 0b1111, 0b1000, 0b1111, 0b1110, 0b1111]
+
+
+def contact_mask_walk_schedule(dt=0.02):
+    """Synthetic schedule through every contact set of ANYmal's four feet (contact_mask_walk_events over MASK_WALK), three
+    time steps per phase.  Asserts its own coverage: every mask on at least two Intermediate grid points, every single-foot
+    impact, switching constraints of dimension 3, 6, 9 and 12, and impacts that also lift a foot."""
+    ev = contact_mask_walk_events(MASK_WALK, dt)
+    N = 3 * len(MASK_WALK) + 1
+    td = TimeDiscretization(N * dt, N).discretize(ev, 0.0, sto=False)
+    ctrl = stage_ctrl_array(td, ev)
+    per_mask = np.bincount([c.contact_mask for c in ctrl if c.type == 0], minlength=16)
+    assert per_mask.min() >= 2, per_mask
+    impacts = [i for i, c in enumerate(ctrl) if c.type == IMPACT]
+    assert {0b0001, 0b0010, 0b0100, 0b1000} <= {ctrl[i].contact_mask for i in impacts}
+    assert {c.ns for c in ctrl} == {0, 3, 6, 9, 12}
+    assert {c.nf for c in ctrl} == {0, 3, 6, 9, 12}
+    assert sum(1 for i in impacts if ctrl[i - 1].contact_mask & ~ctrl[i + 1].contact_mask) >= 2  # land one foot, lift another
+    return td, ev, ctrl
 
 
 def dense_kkt_solve(dims, L, ctrl, kkt1, dx0):

@@ -262,6 +262,38 @@ def anymal_trot_events() -> ContactEvents:
     return ev
 
 
+def anymal_crawl_events(sto: bool = False) -> ContactEvents:
+    """One cycle of the contact schedule of robotoc/examples/anymal/crawl.cpp:161-210 (contact order LF, LH, RF, RH, bit per
+    contact as in anymal_trot_events): one foot swings at a time, so the stances have three feet (dimf 9) and every impact
+    closes a single foot (impact dimf 3).  At t0 + swing RH lands while RF lifts, at t0 + ds + 3 swing LH lands while LF
+    lifts: impacts whose post-impact contact set also drops a contact."""
+    ev = ContactEvents(phase_dimf=[12], phase_mask=[0b1111])
+    t0, swing, ds = 0.04, 0.5, 0.04
+    ev.push_back(False, t0, 9, sto=sto, post_mask=0b0111)                                          # RH swings
+    ev.push_back(True, t0 + swing, 9, impact_dimf=3, sto=sto, post_mask=0b1011, impact_mask=0b1000)  # RH lands, RF swings
+    ev.push_back(True, t0 + 2 * swing, 12, impact_dimf=3, sto=sto, post_mask=0b1111, impact_mask=0b0100)
+    ev.push_back(False, t0 + 2 * swing + ds, 9, sto=sto, post_mask=0b1101)                         # LH swings
+    ev.push_back(True, t0 + 3 * swing + ds, 9, impact_dimf=3, sto=sto, post_mask=0b1110, impact_mask=0b0010)  # LH lands, LF swings
+    ev.push_back(True, t0 + 4 * swing + ds, 12, impact_dimf=3, sto=sto, post_mask=0b1111, impact_mask=0b0001)
+    return ev
+
+
+def contact_mask_walk_events(masks, dt: float) -> ContactEvents:
+    """Synthetic schedule that walks through the contact sets `masks` (one phase each, three time steps long, events in the
+    middle of a time step): an event is an impact iff it closes a contact, and an impact that also opens one is both."""
+    ev = ContactEvents(phase_dimf=[3 * bin(masks[0]).count("1")], phase_mask=[masks[0]])
+    for k in range(1, len(masks)):
+        pre, post = masks[k - 1], masks[k]
+        closed = post & ~pre
+        t = (3 * k + 0.5) * dt
+        dimf = 3 * bin(post).count("1")
+        if closed:
+            ev.push_back(True, t, dimf, impact_dimf=3 * bin(closed).count("1"), post_mask=post, impact_mask=closed)
+        else:
+            ev.push_back(False, t, dimf, post_mask=post)
+    return ev
+
+
 def anymal_jump_sto_events() -> ContactEvents:
     """Contact schedule of robotoc/examples/anymal/jump_sto.cpp:42-48,131-140:
     stand(12) -lift@0.4 (sto)-> flying(0) -impact@0.9 (sto)-> stand; T=1.7."""

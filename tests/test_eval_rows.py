@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import oracle_lib
-from helpers import jump_sto_schedule, small_event_schedule, trot_schedule
+from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, small_event_schedule, trot_schedule
 from robotoc_b200 import ANYMAL, StageDims, StageLayout, anymal_constraint_table
 from robotoc_b200.grid import IMPACT, TERMINAL
 from synth import make_stage_inputs, mat
@@ -122,11 +122,13 @@ def test_oracle_set_slack_and_dual_positive_and_initial_state_direction():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("which,batch", [("small_sto", 3), ("trot", 16), ("jump", 4), ("trot_icone", 5)])
+@pytest.mark.parametrize("which,batch", [("small_sto", 3), ("trot", 16), ("jump", 4), ("trot_icone", 5), ("crawl_icone", 4),
+                                         ("mask_walk", 3)])
 def test_cuda_eval_rows_match_the_oracle(which, batch):
     from robotoc_b200 import DirectMultipleShooting, RiccatiRecursion
-    sched = {"small_sto": small_event_schedule(True), "trot": trot_schedule(40), "jump": jump_sto_schedule(80),
-             "trot_icone": trot_schedule(40)}[which]
+    sched = {"small_sto": lambda: small_event_schedule(True), "trot": lambda: trot_schedule(40), "jump": lambda: jump_sto_schedule(80),
+             "trot_icone": lambda: trot_schedule(40), "crawl_icone": lambda: crawl_schedule(54),
+             "mask_walk": contact_mask_walk_schedule}[which]()
     lib, table, sd, S, ctrl, lin, con, sol, dx0 = _setup(sched, batch, 63, getter=None, impact_cones=which.endswith("icone"))
     S = StageLayout(sd)
     rr = RiccatiRecursion(ANYMAL, len(ctrl), batch)

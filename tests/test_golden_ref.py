@@ -54,15 +54,17 @@ GL = load(mgl.PATH)
 
 @pytest.mark.parametrize("name,seed", mgl.RICCATI_CASES)
 def test_oracle_equals_live_reference_every_field(name, seed):
-    """Every field of every Riccati / direction record and the mutated KKT blocks (F, H, G, lu'), batch 3, fresh seeds."""
+    """Every field of every Riccati / direction record and the mutated KKT blocks (F, H, G, lu'), batch 3, fresh seeds; the
+    crawl cases (golden_ref_gaits.npz) add stages with three contacts, single-foot impacts and ns = 3."""
     from synth import make_kkt
     lib = oracle_lib.load()
     L = Layout(ANYMAL, getter=lib.orc_layout_get)
-    td, ev, ctrl = mg.CASES[name][0]()
+    td, ev, ctrl = mgl.schedule(name)
     kkt, dx0 = make_kkt(ANYMAL, L, ctrl, batch=3, seed=seed)
     kk_o, ric_o, d_o, info = oracle_lib.riccati_batch(ANYMAL, L, ctrl, kkt, dx0)
     assert info == 0
-    kk_r, ric_r, d_r = (restore(GL, f"ric_{name}_{k}", a) for k, a in (("kkt", kk_o), ("ric", ric_o), ("dir", d_o)))
+    G_case = GL if mgl.fixture_path(name) == mgl.PATH else load(mgl.fixture_path(name))
+    kk_r, ric_r, d_r = (restore(G_case, f"ric_{name}_{k}", a) for k, a in (("kkt", kk_o), ("ric", ric_o), ("dir", d_o)))
     fields = sorted((getattr(L, f), f) for f in mgl.RIC_FIELDS)
     ends = [o for o, _ in fields[1:]] + [L.r_stosc + 2]
     for (o, f), e in zip(fields, ends):

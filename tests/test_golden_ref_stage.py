@@ -127,7 +127,7 @@ def test_oracle_equals_live_reference_stage_layer(which, seed):
     lib = oracle_lib.load()
     table, sd, S, K, ctrl, lin, con, sol, dx0, icone = mgl.stage_case(which, seed, lib.orc_stage_layout_get, lib.orc_layout_get)
     got = oracle_iteration(sd, S, K, table, ctrl, lin, con, sol, dx0)
-    GL = load(mgl.PATH)
+    GL = load(mgl.fixture_path(which))
     ref = {k: restore(GL, f"stage_{which}_{k}", got[k]) for k in mgl.STAGE_KEYS}
     _cmp_records(S, K, ctrl, got, ref, TOL, impact_cones=icone)
 
@@ -145,6 +145,13 @@ def test_cuda_reproduces_the_reference_iteration_golden(impact_cones):
     pref = (G["ic_perf_stage"] if impact_cones else G["perf_stage"]).sum(axis=1)
     np.testing.assert_allclose(perf[:, 1:5], pref, rtol=1e-11)
     np.testing.assert_allclose(perf[:, 5], np.sqrt(pref[:, 3]), rtol=1e-11)
+    got = _cuda_iteration(rr, dms, S, lin, con, sol, dx0)
+    _cmp_records(S, K, ctrl, got, _golden(got, impact_cones), 1e-8, impact_cones=impact_cones)
+    rr.close()
+
+
+def _cuda_iteration(rr, dms, S, lin, con, sol, dx0):
+    """One iteration through the C ABI, every record the reference iteration stores."""
     dms.condense(lin, con)
     got = dict(kkt=dms.getKKT(), cc_cond=dms.getConstraintData())
     rr.backwardRiccatiRecursion()
@@ -157,5 +164,20 @@ def test_cuda_reproduces_the_reference_iteration_golden(impact_cones):
     dms.integrateSolution(sol)
     got["d_upd"], got["xd_upd"], got["cc_upd"], got["ex_upd"] = (rr.getDirection(), dms.getExpandedDirection(), dms.getConstraintData(),
                                                                  reference_view_of_expansion(S, dms.getExpansionData()))
-    _cmp_records(S, K, ctrl, got, _golden(got, impact_cones), 1e-8, impact_cones=impact_cones)
+    return got
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("which,seed", [(w, s) for w, s in mgl.STAGE_CASES if w in mgl.GAIT_CASES])
+def test_cuda_reproduces_the_reference_iteration_gaits(which, seed):
+    """The CUDA iteration against the reference's own on the crawl (with / without switching-time optimisation and impact
+    cones) and contact-mask-walk schedules (golden_ref_gaits.npz)."""
+    from robotoc_b200 import ANYMAL, DirectMultipleShooting, RiccatiRecursion
+    table, sd, S, K, ctrl, lin, con, sol, dx0, icone = mgl.stage_case(which, seed, None, None)
+    rr = RiccatiRecursion(ANYMAL, len(ctrl), lin.shape[0])
+    rr.setTimeDiscretization(ctrl)
+    got = _cuda_iteration(rr, DirectMultipleShooting(rr, sd, table), S, lin, con, sol, dx0)
+    GL = load(mgl.GAITS_PATH)
+    _cmp_records(S, K, ctrl, got, {k: restore(GL, f"stage_{which}_{k}", got[k]) for k in mgl.STAGE_KEYS if k in got},
+                 1e-8, impact_cones=icone)
     rr.close()

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import oracle_lib
-from helpers import jump_sto_schedule, rel_err, trot_schedule
+from helpers import crawl_schedule, jump_sto_schedule, rel_err, trot_schedule
 from iteration_check import compare_final, oracle_iteration, oracle_sensitivity, run_device_iteration
 from robotoc_b200 import (ANYMAL, DirectMultipleShooting, Layout, RiccatiRecursion, StageDims, StageLayout, ULayout,
                           UnconstrRiccatiRecursion, anymal_constraint_table)
@@ -59,6 +59,13 @@ def test_config4_jump_sto_n80_batch512_full_iteration():
     td, ev, ctrl = jump_sto_schedule(80)
     assert len(ctrl) == 84 and any(c.sto for c in ctrl)
     print("worst rel err", _full_iteration(ctrl, 512, 20260931))
+
+
+def test_crawl_n54_batch1024_full_iteration():
+    """The crawl schedule (three-foot stances, single-foot impacts, ns = 3) at the trot config's batch size."""
+    td, ev, ctrl = crawl_schedule(54)
+    assert len(ctrl) == 61
+    print("worst rel err", _full_iteration(ctrl, 1024, 20260935))
 
 
 def test_config3_trot_n40_batch1024_riccati_api():

@@ -4,9 +4,10 @@ import numpy as np
 import pytest
 
 import oracle_lib
-from helpers import jump_sto_schedule, rel_err, small_event_schedule, trot_schedule
+from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, rel_err, small_event_schedule, trot_schedule
 from robotoc_b200 import ANYMAL, Layout, RiccatiRecursion, ULayout, UnconstrRiccatiRecursion
-from robotoc_b200.grid import IMPACT
+from robotoc_b200 import _lib
+from robotoc_b200.grid import IMPACT, INTERMEDIATE
 from synth import make_kkt, make_unconstr_kkt
 
 pytestmark = pytest.mark.gpu
@@ -120,6 +121,64 @@ def test_jump_sto_n80_config4_small_batch():
     assert len(ctrl) == 84
     w = _run_case(ctrl, batch=3, seed=20260928)
     print("worst rel err", w)
+
+
+@pytest.mark.parametrize("which,batch,seed", [("crawl", 5, 20260940), ("crawl_sto", 4, 20260941), ("mask_walk", 3, 20260942)])
+def test_gait_schedules(which, batch, seed):
+    """Crawl (nf = 3 / 9, ns = 3 switching constraints, impacts that also lift a foot), with and without switching-time
+    optimisation, and the walk through all 16 contact masks (ns = 3, 6, 9, 12 through the NS = 12 Schur path)."""
+    td, ev, ctrl = {"crawl": lambda: crawl_schedule(54), "crawl_sto": lambda: crawl_schedule(54, sto=True),
+                    "mask_walk": contact_mask_walk_schedule}[which]()
+    w = _run_case(ctrl, batch=batch, seed=seed)
+    print("worst rel err", w)
+
+
+RBT_FXX_AUTO, RBT_FXX_MECHANICAL, RBT_FXX_GENERAL = 0, 1, 2  # include/robotoc_b200.h
+
+
+def test_backward_instance_selection_on_a_mixed_batch():
+    """The backward sweep has an instance for Fxx with the mechanical structure (Fqq = I, Fqv = dt I outside the floating-base
+    blocks) and a general one; with RBT_FXX_AUTO the uploaded records are inspected on the device.  One entry of ONE OCP in the
+    middle of the batch breaks the structure: every OCP must still match the oracle.  On conforming records the forced general
+    instance agrees with AUTO to rounding, and the declared structure gives AUTO's bits."""
+    td, ev, ctrl = crawl_schedule(54)
+    dims, L = ANYMAL, Layout(ANYMAL)
+    nx, batch = dims.nx, 7
+    kkt, dx0 = make_kkt(dims, L, ctrl, batch=batch, seed=20260943)
+    lib = _lib.lib()
+    rr = RiccatiRecursion(dims, len(ctrl), batch)
+    rr.setTimeDiscretization(ctrl)
+
+    def solve(mode, k):
+        assert lib.rbt_set_fxx_structure(rr._h, mode) == 0
+        rr.backwardRiccatiRecursion(k, write_fact=True)
+        rr.forwardRiccatiRecursion(dx0)
+        assert int(rr.info().max()) == 0
+        return rr.getRiccatiFactorization(), rr.getDirection(), rr.getFactorizedKKT()
+
+    auto = solve(RBT_FXX_AUTO, kkt)
+    for a, b in zip(solve(RBT_FXX_MECHANICAL, kkt), auto):
+        np.testing.assert_array_equal(a, b)
+    gen = solve(RBT_FXX_GENERAL, kkt)
+    assert rel_err(gen[0], auto[0]) < 1e-12 and rel_err(gen[1], auto[1]) < 1e-12
+    for i, c in enumerate(ctrl[:-1]):  # the factorized KKT blocks the sweep writes
+        for fo, n in ((L.f_F, nx * nx),) + (((L.f_H, nx * dims.nu), (L.f_G, dims.nu ** 2), (L.f_lu, dims.nu)) if c.type != IMPACT else ()):
+            assert rel_err(gen[2][:, i, fo:fo + n], auto[2][:, i, fo:fo + n]) < 1e-12, f"stage {i}"
+    # one Fqq entry of a leg joint row (rows NP..NV-1) of OCP 4, at a middle Intermediate stage
+    ob, i = 4, next(i for i in range(len(ctrl) // 2, len(ctrl)) if ctrl[i].type == INTERMEDIATE)
+    bad = kkt.copy()
+    bad[ob, i, L.k_Fxx + 10 + 3 * nx] = 0.05
+    kk, ric_o, d_o, info = oracle_lib.riccati_batch(dims, L, ctrl, bad, dx0)
+    assert info == 0
+    ric, d, f = solve(RBT_FXX_AUTO, bad)
+    w = _compare(dims, L, ctrl, ric, ric_o, d, d_o, f, kk)
+    print("worst rel err", w)
+    # the entry matters: the structured instance, wrongly declared, misses it on that OCP only
+    ric_m = solve(RBT_FXX_MECHANICAL, bad)[0]
+    assert rel_err(ric_m[ob, :i + 1], ric_o[ob, :i + 1]) > 1e-6
+    assert rel_err(np.delete(ric_m, ob, 0), np.delete(ric, ob, 0)) < 1e-12
+    assert lib.rbt_set_fxx_structure(rr._h, RBT_FXX_AUTO) == 0
+    rr.close()
 
 
 @pytest.mark.parametrize("N,batch,dt", [(20, 1, 0.05), (50, 16, 0.02)])

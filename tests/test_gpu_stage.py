@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import oracle_lib
-from helpers import jump_sto_schedule, rel_err, small_event_schedule, trot_schedule
+from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, rel_err, small_event_schedule, trot_schedule
 from robotoc_b200 import ANYMAL, DirectMultipleShooting, Layout, RiccatiRecursion, StageDims, StageLayout, anymal_constraint_table
 from robotoc_b200.grid import IMPACT, TERMINAL
 from synth import make_stage_inputs, robotoc_cost_structure, symmetrize_lin
@@ -204,3 +204,58 @@ def test_stage_layer_single_ocp_with_reserved_grid_points():
     (riccati_recursion.cpp:12-13: N + 1 + reserved_num_discrete_events)."""
     td, ev, ctrl = small_event_schedule(False)
     _run(ctrl, batch=1, seed=25, reserve=4)
+
+
+@pytest.mark.parametrize("which,seed", [("crawl", 28), ("crawl_sto", 29), ("crawl_icone", 30), ("mask_walk", 31)])
+def test_stage_layer_gaits(which, seed):
+    """Contact sets the trot / jump schedules never reach: three-foot stances (nf = 9), single-foot impacts (nf = 3, ns = 3),
+    impacts at which another foot lifts (crawl.cpp), and all 16 contact masks with ns = 3, 6, 9, 12 (mask walk) -- the
+    friction-cone rows and force offsets per mask, the odd-sized J M^-1 J^T Cholesky, the wire segments sized by the active
+    contacts, through every host path."""
+    td, ev, ctrl = {"crawl": lambda: crawl_schedule(54), "crawl_sto": lambda: crawl_schedule(54, sto=True),
+                    "crawl_icone": lambda: crawl_schedule(54), "mask_walk": contact_mask_walk_schedule}[which]()
+    _run(ctrl, batch=2, seed=seed, impact_cones=which.endswith("_icone"))
+
+
+def _iterate(rr, dms, ctrl, lin, con, sol, dx0):
+    """One iteration on the step-by-step path and one through iteration_host_wire, on the schedule `ctrl`."""
+    from iteration_check import run_device_iteration
+    rr.setTimeDiscretization(ctrl)
+    got = run_device_iteration(rr, dms, lin, con, sol, dx0)
+    assert int(got["info"].max()) == 0
+    got["wire"] = dms.iteration_host_wire(dms.pack_wire(lin), lin, con, sol, dx0)
+    return got
+
+
+def test_rescheduling_a_live_handle_matches_fresh_handles():
+    """An MPC loop changes the contact sequence between iterations: crawl -> trot -> crawl on ONE handle (sized for the longest
+    schedule) and one DirectMultipleShooting give the same bits as a fresh handle per schedule -- nothing the previous
+    schedule left behind (wire segment table, box-row table, cached flags, stage-conditional outputs) leaks into the next."""
+    table = anymal_constraint_table()
+    sd = StageDims(ANYMAL, nf_max=12, n_contacts=table.n_contacts, n_box=table.n_box)
+    S = StageLayout(sd)
+    batch = 3
+    crawl, trot = crawl_schedule(54)[2], trot_schedule(40)[2]
+    cases = []
+    for ctrl, seed in ((crawl, 41), (trot, 42)):
+        lin, con, sol, dx0 = make_stage_inputs(sd, S, ctrl, batch, seed)
+        cases.append((ctrl, symmetrize_lin(S, lin), con, sol, dx0))
+    fresh = []
+    for ctrl, lin, con, sol, dx0 in cases:
+        rr = RiccatiRecursion(ANYMAL, len(ctrl), batch)
+        fresh.append(_iterate(rr, DirectMultipleShooting(rr, sd, table), ctrl, lin, con, sol, dx0))
+        rr.close()
+    rr = RiccatiRecursion(ANYMAL, max(len(crawl), len(trot)), batch)
+    dms = DirectMultipleShooting(rr, sd, table)
+    for k in (0, 1, 0):
+        got, want = _iterate(rr, dms, *cases[k]), fresh[k]
+        for key in ("ric", "d", "steps", "sol", "info"):
+            np.testing.assert_array_equal(got[key], want[key], err_msg=f"schedule {k}: {key}")
+        # slack and dual of every row (the derived PDIPM fields of rows a stage does not have are never rewritten: they may
+        # still hold the previous schedule's values, and nothing reads them)
+        for f in ("c_slack", "c_dual"):
+            o = getattr(S, f)
+            np.testing.assert_array_equal(got["cc"][:, :, o:o + S.nc], want["cc"][:, :, o:o + S.nc], err_msg=f"schedule {k}: {f}")
+        for a, b in zip(got["wire"], want["wire"]):
+            np.testing.assert_array_equal(a, b, err_msg=f"schedule {k}: iteration_host_wire")
+    rr.close()

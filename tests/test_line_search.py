@@ -12,7 +12,7 @@ import pytest
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
 import make_golden_ref_live as mgl  # noqa: E402
 import oracle_lib  # noqa: E402
-from helpers import small_event_schedule, trot_schedule
+from helpers import contact_mask_walk_schedule, crawl_schedule, small_event_schedule, trot_schedule
 from iteration_check import oracle_iteration
 from robotoc_b200 import ANYMAL, Layout, StageDims, StageLayout, anymal_constraint_table
 from robotoc_b200.grid import IMPACT, TERMINAL
@@ -116,10 +116,11 @@ def test_oracle_trial_zero_is_the_primal_part_of_the_update(impact_cones):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("which,batch", [("small_sto", 3), ("trot", 8), ("trot_icone", 4)])
+@pytest.mark.parametrize("which,batch", [("small_sto", 3), ("trot", 8), ("trot_icone", 4), ("crawl_icone", 4), ("mask_walk", 3)])
 def test_cuda_line_search_matches_the_oracle(which, batch):
     from robotoc_b200 import DirectMultipleShooting, LineSearch, RiccatiRecursion
-    sched = {"small_sto": small_event_schedule(True), "trot": trot_schedule(40), "trot_icone": trot_schedule(40)}[which]
+    sched = {"small_sto": lambda: small_event_schedule(True), "trot": lambda: trot_schedule(40), "trot_icone": lambda: trot_schedule(40),
+             "crawl_icone": lambda: crawl_schedule(54), "mask_walk": contact_mask_walk_schedule}[which]()
     lib, table, sd, S, K, ctrl, lin, con, sol, dx0, ref = _problem(sched, batch, 72, impact_cones=which.endswith("icone"))
     S = StageLayout(sd)
     rr = RiccatiRecursion(ANYMAL, len(ctrl), batch)

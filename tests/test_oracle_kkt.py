@@ -5,23 +5,21 @@ import numpy as np
 import pytest
 
 import oracle_lib
-from helpers import dense_kkt_solve, dense_kkt_solve_sto, small_event_schedule, rel_err
+from helpers import crawl_schedule, dense_kkt_solve, dense_kkt_solve_sto, small_event_schedule, rel_err
 from robotoc_b200 import ANYMAL, Layout
 from robotoc_b200.grid import IMPACT, LIFT
 from synth import make_kkt
 
 
-@pytest.mark.parametrize("seed", [20260924, 7])
-def test_oracle_direction_solves_full_kkt(seed):
+def _direction_solves_full_kkt(ctrl, batch, seed):
     dims = ANYMAL
     L = Layout(dims)
-    td, ev, ctrl = small_event_schedule(sto=False)
     types = [c.type for c in ctrl]
     assert IMPACT in types and LIFT in types and any(c.ns > 0 for c in ctrl)
-    kkt, dx0 = make_kkt(dims, L, ctrl, batch=2, seed=seed)
+    kkt, dx0 = make_kkt(dims, L, ctrl, batch=batch, seed=seed)
     kk, ric, d, info = oracle_lib.riccati_batch(dims, L, ctrl, kkt, dx0)
     assert info == 0
-    for b in range(2):
+    for b in range(batch):
         ref = dense_kkt_solve(dims, L, ctrl, kkt[b], dx0[b])
         for i in range(len(ctrl)):
             di = d[b, i]
@@ -32,6 +30,20 @@ def test_oracle_direction_solves_full_kkt(seed):
             if ("xi", i) in ref:
                 ns = ctrl[i].ns
                 assert rel_err(di[L.d_dxi:L.d_dxi + ns], ref[("xi", i)]) < 1e-8
+
+
+@pytest.mark.parametrize("seed", [20260924, 7])
+def test_oracle_direction_solves_full_kkt(seed):
+    td, ev, ctrl = small_event_schedule(sto=False)
+    _direction_solves_full_kkt(ctrl, 2, seed)
+
+
+def test_oracle_direction_solves_full_kkt_crawl():
+    """The crawl schedule (the Riccati case of golden_ref_gaits.npz): three-dimensional switching constraints (ns = 3) two grid
+    points before each single-foot impact, and impacts at which another foot lifts."""
+    td, ev, ctrl = crawl_schedule(54)
+    assert {c.ns for c in ctrl} == {0, 3}
+    _direction_solves_full_kkt(ctrl, 1, 35)
 
 
 def test_oracle_riccati_symmetry_and_mutation():
