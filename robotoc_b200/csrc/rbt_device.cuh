@@ -243,8 +243,11 @@ __device__ __forceinline__ bool warp_chol_inv_reg(double (&c)[N], double& rs) {
   return ok;
 }
 
+// Not unrolled: the chain is serial anyway, and with a compile-time n the unrolled loop hoists all 2n loads, which spilled
+// the backward sweep's STO terms (ten chains of up to NX per stage) at its 80-register cap.
 __device__ __forceinline__ double dot_serial(const double* a, const double* b, int n) {
   double s = 0.0;
+#pragma unroll 1
   for (int i = 0; i < n; ++i) s = fma(a[i], b[i], s);
   return s;
 }

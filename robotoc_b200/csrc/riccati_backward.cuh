@@ -177,9 +177,20 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
   const int b = blockIdx.x;
   if (b >= p.batch) return;
   const int N = p.n_grid - 1;
-  const double* kkt_b = p.kkt + size_t(b) * p.n_grid * L.k_stride;
-  double* ric_b = p.ric + size_t(b) * p.n_grid * L.r_stride;
-  double* fact_b = p.fact ? p.fact + size_t(b) * p.n_grid * L.f_stride : nullptr;
+  // Records of grid point st of this OCP, formed from the kernel parameters where they are used: three 64-bit base pointers
+  // held across the stage loop cost six registers, and the loop runs at the 80-register cap of 4 CTAs per SM.
+  const int bst = b * p.n_grid;
+  auto kkt_at = [&](int st) { return p.kkt + size_t(bst + st) * L.k_stride; };
+  auto ric_at = [&](int st) { return p.ric + size_t(bst + st) * L.r_stride; };
+
+  // The accumulator fragments cF and cH belong to the GEMM warps and are only defined and read under role branches.  The compiler cannot tell that `gemm_warp` is the same in every branch, so an array left
+  // undefined on the other role's path is live there as well, around the stage loop: that spilled the sweep.  Every path
+  // that ends a role branch without the array therefore gives it a fresh (zero) value, which ends the old live range.
+  auto end_live_range = [](auto& frag) {
+    double* v = &frag[0][0];
+#pragma unroll
+    for (int k = 0; k < int(sizeof(frag) / sizeof(double)); ++k) v[k] = 0.0;
+  };
 
   const double* sFx = sIn + (L.k_Fx - L.k_Fxx);
   const double* slx = sIn + (L.k_lx - L.k_Fxx);
@@ -232,7 +243,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
   auto issue_stage_load = [&](int st) {
     // one elected thread: stage st's [Fxx|Fvu|Fx|lx|lu] (+ extras when flagged)
     const rbt_stage_ctrl cs = p.ctrl[st];
-    const double* rec = kkt_b + size_t(st) * L.k_stride;
+    const double* rec = kkt_at(st);
     fence_proxy_async();
     mbar_expect_tx(&bars[0], uint32_t(L.k_stage_size) * 8u);
     tma_load_1d(sIn, rec + L.k_Fxx, uint32_t(L.k_stage_size) * 8u, &bars[0]);
@@ -262,8 +273,8 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
 
   // ---- terminal stage: P_N = Qxx_N, s_N = -lx_N          riccati_recursion.cpp:37-38
   {
-    const double* recN = kkt_b + size_t(N) * L.k_stride;
-    double* ricN = ric_b + size_t(N) * L.r_stride;
+    const double* recN = kkt_at(N);
+    double* ricN = ric_at(N);
     for (int e = tid; e < NX * NX; e += NTHR) {
       const double v = recN[L.k_Qxx + e];
       sP[e] = v;
@@ -289,9 +300,9 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
     const bool sto = cs.sto != 0, sto_next = cs.sto_next != 0;
     const bool extras = (cs.ns > 0 || cs.sto);
     const bool plain = !impact && ns == 0;  // factor-warp fast path
-    const double* rec = kkt_b + size_t(i) * L.k_stride;
-    double* ric = ric_b + size_t(i) * L.r_stride;
-    double* fct = fact_b ? fact_b + size_t(i) * L.f_stride : nullptr;
+    const double* rec = kkt_at(i);
+    double* ric = ric_at(i);
+    double* fct = p.fact ? p.fact + size_t(bst + i) * L.f_stride : nullptr;
 
     // ---- phase transition on the in-shared "next" factorization     riccati_recursion.cpp:42-62, riccati_factorizer.cpp:145-175
     {
@@ -302,7 +313,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
         pol = ric;
       } else if (p.ctrl[i + 1].type == RBT_LIFT) {
         do_pt = sto || sto_next;
-        pol = ric_b + size_t(i + 1) * L.r_stride;
+        pol = ric_at(i + 1);
       }
       if (do_pt) {
         const double xi = scn[0], chi = scn[1], rho = scn[2], eta = scn[3], iota = scn[4];
@@ -358,19 +369,6 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
     auto rho_of = [](int k) { return k < NP ? k : k - NP + NV; };
     // STRUCT: rows NP..NV-1 of Fxx are [e_rho^T, dt e_rho^T] (structural); rows {0..NP-1} and {NV..2NV-1} are contracted
     // in full (K = KR = NP + NV), the structural rows contribute a shifted copy of the other operand.
-
-    // factor warp: Quu -> accumulator fragments of G, issued before it parks at the Bp barrier (L2 latency off its chain)
-    double cG[TU][TU][2];
-    if (!gemm_warp && !impact) {
-#pragma unroll
-      for (int ub = 0; ub < TU; ++ub)
-#pragma unroll
-        for (int n = 0; n < TU; ++n) {
-          const int u0 = tile_off(ub, NU), v0 = tile_off(n, NU);
-          cG[ub][n][0] = __ldg(rec + L.k_Quu + (u0 + g) + (v0 + 2 * t) * NU);
-          cG[ub][n][1] = __ldg(rec + L.k_Quu + (u0 + g) + (v0 + 2 * t + 1) * NU);
-        }
-    }
 
     // ---- wait for this stage's blocks
     RBT_TL(i, 0);
@@ -447,6 +445,8 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
           cH[n][0] = __ldg(rec + L.k_Qxu + (i0 + g) + (u0 + 2 * t) * NX);
           cH[n][1] = __ldg(rec + L.k_Qxu + (i0 + g) + (u0 + 2 * t + 1) * NX);
         }
+      } else {
+        end_live_range(cH);
       }
       matvec_N4(sP, NX, NX, NX, sFx, tid, NG, [&](int r, double a) { z[r] = s_n[r] - a; });
       if (sto) {
@@ -527,6 +527,17 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
     } else {
       // ================= factor warp: G = Quu + (Bv^T P+_vv) Bv, then L (G = L L^T) and L^-1 in registers
       if (!impact) {
+        // Quu -> accumulator fragments of G, issued before the warp parks at the Bp barrier (L2 latency off its chain).  Not
+        // before the stage wait: all warps pass that wait, and 16 registers of G in flight there made it the kernel's peak.
+        double cG[TU][TU][2];
+#pragma unroll
+        for (int ub = 0; ub < TU; ++ub)
+#pragma unroll
+          for (int n = 0; n < TU; ++n) {
+            const int u0 = tile_off(ub, NU), v0 = tile_off(n, NU);
+            cG[ub][n][0] = __ldg(rec + L.k_Quu + (u0 + g) + (v0 + 2 * t) * NU);
+            cG[ub][n][1] = __ldg(rec + L.k_Quu + (u0 + g) + (v0 + 2 * t + 1) * NU);
+          }
         named_bar_sync(3, NTHR);  // Bp = Bv^T P+[nv:, nv:] from the GEMM warps
         RBT_TL(i, 2);
 #pragma unroll
@@ -570,6 +581,8 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
         }
         RBT_TL(i, 4);
       }
+      end_live_range(cF);
+      end_live_range(cH);
     }
     RBT_TL(i, 7);
     if (tid == 0) tma_store_wait_read();  // the previous stage's bulk store of P has long read shared memory (issued a whole stage ago)
@@ -689,6 +702,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
               ric[L.r_W + lane] = sto_next ? -bq : 0.0;
             }
           }
+          end_live_range(cF);
         }
       } else {
         // ================= Schur-complement path (switching constraint)      riccati_factorizer.cpp:58-89
@@ -708,6 +722,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
         __syncthreads();
         if (!gemm_warp) {
           if (!warp_cholesky<NU>(sG, NU, dinv)) bad |= 1;
+          end_live_range(cF);
         }
         __syncthreads();
         if (tid < NU) chol_solve_smem(sG, dinv, NU, Ginv + tid * NU, 1);            // Ginv = G^-1             :60
@@ -726,6 +741,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
         __syncthreads();
         if (!gemm_warp) {
           if (!warp_cholesky<NS>(Sm, ns, dinvS)) bad |= 2;
+          end_live_range(cF);
         }
         __syncthreads();
         // SDG = S^-1 DGinv (:65);  M = S^-1 C (:71);  m = S^-1 p (:73);  mt = S^-1 Phit (:116)
@@ -996,10 +1012,10 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
       double sgm = xi - 2.0 * chi + rho;
       if ((sgm * p.max_dts0) < fabs(eta - iota) || sgm < 1.4901161193847656e-08) sgm = fabs(sgm) + fabs(eta - iota) / p.max_dts0;
       const double is = 1.0 / sgm;
-      if (tid < NX) ric_b[L.r_dtsdx + tid] = -is * (Psin[tid] - Phin[tid]);
+      if (tid < NX) ric_at(0)[L.r_dtsdx + tid] = -is * (Psin[tid] - Phin[tid]);
       if (tid == 0) {
-        ric_b[L.r_stosc + 0] = is * (xi - chi);
-        ric_b[L.r_stosc + 1] = -is * (eta - iota);
+        ric_at(0)[L.r_stosc + 0] = is * (xi - chi);
+        ric_at(0)[L.r_stosc + 1] = -is * (eta - iota);
       }
     }
   }

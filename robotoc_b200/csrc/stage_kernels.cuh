@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(32 * MjtjCfg<NV, NFM>::WARPS, 10) mjtjinv_kern
 // ------------------------------------------------------------------------------------------------------------------
 // K2: everything else of "Forms linear system", with all dense products on the fp64 tensor pipe (DMMA m8n8k4).
 //
-// Shared-memory plan (35.8 KB -> 6 CTAs per SM).  The parts of the linearization record K2 needs are contiguous
+// Shared-memory plan (35.8 KB: room for 6 CTAs per SM; the launch bounds below allow 5).  The parts of the linearization record K2 needs are contiguous
 // ([l_D, l_Qxx), [l_Quu, l_Phix) and [l_ha, l_dgdq)), so they land IN PLACE with three cp.async.bulk copies and are then
 // used (and modified: PDIPM terms) where they lie; Z (from K1) is a fourth copy; the PDIPM inputs (slack|dual|res,
 // dg/dq|dg/df) land in the buffer that later holds R.  The cost Hessian Qxx is NOT staged: it is only the accumulator
@@ -337,8 +337,10 @@ struct CondCfg {
   static_assert((NFM * NX) % 2 == 0 && (NFM * NV) % 2 == 0, "Qaf | Quf are adjacent in the expansion record (one bulk store)");
 };
 
+// 5 CTAs per SM (72 registers, no spill) measured faster on H100 than 6 (64 registers, spills in the phase-5 products) and
+// no slower than 4: DESIGN.md 3.4.
 #ifndef RBT_COND_MIN_CTAS
-#define RBT_COND_MIN_CTAS 6
+#define RBT_COND_MIN_CTAS 5
 #endif
 template <int NV, int NU, int NFM>
 __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_CTAS) condense_kernel(const StageParams p) {
@@ -881,6 +883,7 @@ __global__ void __launch_bounds__(CondCfg<NV, NU, NFM>::NTHREADS, RBT_COND_MIN_C
     });
     for (int ii = tid; ii < NU; ii += NTHR) {
       double acc = 0.0;
+#pragma unroll 1  // a serial chain: unrolled, its 2 NVF hoisted loads were the kernel's spill frame
       for (int l = 0; l < NVF; ++l) acc = fma(sZ[(np + ii) + l * NVF], vhaf[l], acc);
       kkt[K.k_hu + ii] = (vhu[ii] + acc) * g1;
     }
