@@ -109,6 +109,17 @@ int rbt_check_info(rbt_handle* h, int* first_bad, void* stream);
 enum { RBT_FXX_AUTO = 0, RBT_FXX_MECHANICAL = 1, RBT_FXX_GENERAL = 2 };
 int rbt_set_fxx_structure(rbt_handle* h, int mode);
 
+/* Time-parallel Riccati sweeps.  Without switching-time optimisation the backward sweep carries only (P, s) from grid i+1 to
+ * grid i and the forward sweep only dx (src/riccati/riccati_recursion.cpp:32-131 with every sto flag false), so the horizon
+ * can be split into `segments` contiguous pieces that run on separate CTAs: the (P, s) at every segment end comes from an
+ * associative combine of per-stage value-function elements and dx at every segment start from composed closed-loop maps,
+ * then each segment runs the serial per-stage algebra.  Same outputs up to rounding; worth it only when the batch leaves
+ * most SMs idle.  0 = automatic (default: chosen from the handle's batch, the SM count and the schedule), 1 = serial,
+ * k > 1 = k segments.  Returns RBT_ERR_ARG for k > n_grid - 1 of the current schedule (set the schedule first) or for k > 1 on
+ * a schedule with switching-time optimisation; such schedules always run serially, and a later schedule with fewer stages
+ * clamps k.  Applies to rbt_riccati_backward / forward and every host path built on them. */
+int rbt_set_time_segments(rbt_handle* h, int segments);
+
 /* RiccatiRecursion::backwardRiccatiRecursion(time_discretization, kkt_matrix, kkt_residual, factorization)
  *   src/riccati/riccati_recursion.cpp:32-80.  Reads RBT_BUF_KKT, writes RBT_BUF_RIC (P,s,K,k,M,m,STO terms,
  *   STOPolicy) and, if write_fact != 0, RBT_BUF_FACT (the values the reference leaves in Qxx,Qxu,Quu,lu). */

@@ -139,6 +139,14 @@ class RiccatiRecursion {
     max_dts0_ = max_dts0;
   }
 
+  /// Time-parallel sweeps (rbt_set_time_segments): 0 = automatic (default), 1 = serial, k > 1 = k segments of the horizon on
+  /// separate CTAs.  Checked against the time discretization of every following sweep: k > 1 throws std::invalid_argument on
+  /// a horizon with fewer than k stages or with switching-time optimisation.
+  void setTimeSegments(int segments) {
+    if (segments < 0) throw std::invalid_argument("[RiccatiRecursion] invalid argument: 'segments' must be non-negative!");
+    segments_ = segments;
+  }
+
   /// riccati_recursion.cpp:32-80.  kkt_matrix / kkt_residual are mutated like the reference (Qxx,Qxu,Quu,lu <- F,H,G,lu').
   void backwardRiccatiRecursion(const TimeDiscretization& td, KKTMatrix& kkt_matrix, KKTResidual& kkt_residual,
                                 RiccatiFactorization& factorization) {
@@ -268,12 +276,14 @@ class RiccatiRecursion {
       c.dt = td[i].dt;
     }
     check(rbt_set_schedule(h_, ctrl_.data(), int(td.size()), max_dts0_));
+    check(rbt_set_time_segments(h_, segments_));
   }
 
   rbt_dims dims_;
   rbt_layout L_;
   int n_grid_max_;
   double max_dts0_;
+  int segments_ = 0;
   rbt_handle* h_ = nullptr;
   std::vector<rbt_stage_ctrl> ctrl_;
   std::vector<LQRPolicy> lqr_policy_;

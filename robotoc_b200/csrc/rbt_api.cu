@@ -16,6 +16,7 @@
 #include "../../include/robotoc_b200.h"
 #include "riccati_backward.cuh"
 #include "riccati_forward.cuh"
+#include "riccati_time_parallel.cuh"
 #include "riccati_unconstr.cuh"
 #include "stage_kernels.cuh"
 #include "ustage_kernels.cuh"
@@ -57,6 +58,12 @@ struct rbt_handle {
   int* d_arrivals = nullptr;  // per-SM CTA arrival counters (CTA de-phasing in the backward kernel)
   int* d_struct = nullptr;    // [0]: 1 = every Fxx of the KKT buffer has the mechanical structure (see rbt_set_fxx_structure)
   int fxx_mode = RBT_FXX_AUTO;
+  // time-parallel sweeps (riccati_time_parallel.cuh): requested segment count (0 = automatic, 1 = serial) and scratch,
+  // allocated on the first segmented sweep; the S-dependent buffers grow with the largest S used
+  int tsegs = 0, n_sm = 0, tp_cap = 0;
+  double *d_tp_elem = nullptr, *d_tp_scan[2] = {nullptr, nullptr}, *d_tp_fmap = nullptr, *d_tp_dx = nullptr;
+  int* d_tp_fail = nullptr;
+  const double* tp_seeds = nullptr;  // the scan buffer the last segmented backward sweep read its seeds from
   bool kkt_from_condense = false;  // the KKT records were just written by rbt_condense: structure holds by construction
   int stagger_ns = 0;
   long long* d_timeline = nullptr;  // bring-up instrumentation (RBT_TIMELINE_CTA)
@@ -90,7 +97,7 @@ struct rbt_handle {
   long long w_ocp = 0;               // doubles of one OCP's concatenated wire records
   int cost_structure = RBT_COST_GENERAL;  // what the host's wire records hold (rbt_set_wire_cost_structure)
   bool wire_dirty = true;                 // per-grid-point wire layouts on the device are stale (schedule / cost structure changed)
-  bool attr_bwd = false, attr_fwd = false, attr_cond = false;  // MaxDynamicSharedMemorySize set on THIS handle's device
+  bool attr_bwd = false, attr_fwd = false, attr_cond = false, attr_tp = false;  // MaxDynamicSharedMemorySize set on THIS handle's device
   cudaEvent_t ev_condense_mid = nullptr;  // caller-owned event recorded between the two kernels of rbt_condense (timing)
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   std::vector<cudaEvent_t> ev;
@@ -194,6 +201,7 @@ int rbt_create(const rbt_dims* dims, int n_grid_max, int batch, int device, rbt_
   RBT_CUDA(h, cudaMemset(h->d_fact, 0, per * h->L.f_stride * 8));
   RBT_CUDA(h, cudaMemset(h->d_dir, 0, per * h->L.d_stride * 8));
   RBT_CUDA(h, cudaMemset(h->d_info, 0, size_t(batch) * sizeof(int)));
+  RBT_CUDA(h, cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device));
   return RBT_OK;
 }
 
@@ -241,6 +249,8 @@ int rbt_destroy(rbt_handle* h) {
   cudaFree(h->d_stage_perf);
   cudaFree(h->d_perf);
   cudaFree(h->d_x0in);
+  cudaFree(h->d_tp_elem); cudaFree(h->d_tp_scan[0]); cudaFree(h->d_tp_scan[1]); cudaFree(h->d_tp_fmap); cudaFree(h->d_tp_dx);
+  cudaFree(h->d_tp_fail);
   delete h;
   return RBT_OK;
 }
@@ -502,6 +512,129 @@ int rbt_check_info(rbt_handle* h, int* first_bad, void* stream) {
   return RBT_OK;
 }
 
+// ---- time-parallel sweeps (riccati_time_parallel.cuh) ------------------------------------------------------------------
+// Segment count of the next sweep: 1 (serial) on any schedule with switching-time optimisation, whose phase transitions are
+// serial; otherwise the request of rbt_set_time_segments (clamped to N), or the automatic choice from the HANDLE's batch (not
+// the chunk a pipelined host path works on), so one handle always takes the same path at every chunk size.
+static int tp_auto_segments(int batch, int n_sm, int N) {
+  // Serial everywhere: on an H100 SXM (BASELINE.md section 6, tools/time_parallel_latency.py) the segmented sweeps were
+  // faster at no batch size from 1 to 1024 and no segment count from 2 to N (at batch 1 the best, S = 23, ties the serial
+  // sweeps).  Kept as the one place where a faster combine would enable them.
+  (void)batch; (void)n_sm; (void)N;
+  return 1;
+}
+
+static int tp_segments(const rbt_handle* h) {
+  const int N = h->n_grid - 1;
+  if (N < 2 || ctrl_has_sto(h->ctrl.data(), h->n_grid)) return 1;
+  if (h->tsegs == 1) return 1;
+  if (h->tsegs > 1) return std::min(h->tsegs, N);
+  return std::min(tp_auto_segments(h->batch, h->n_sm, N), N);
+}
+
+int rbt_set_time_segments(rbt_handle* h, int segments) {
+  if (!h || segments < 0) return RBT_ERR_ARG;
+  if (segments > 1) {
+    if (segments > h->n_grid - 1) {
+      h->err = "[rbt_set_time_segments] invalid argument: more segments than stages (set the schedule first)";
+      return RBT_ERR_ARG;
+    }
+    if (ctrl_has_sto(h->ctrl.data(), h->n_grid)) {
+      h->err = "[rbt_set_time_segments] invalid argument: a schedule with switching-time optimisation is swept serially";
+      return RBT_ERR_ARG;
+    }
+  }
+  h->tsegs = segments;
+  return RBT_OK;
+}
+
+static int tp_ensure(rbt_handle* h, int S) {
+  const size_t esz = rbt::TpElem<2 * 18>::SIZE;  // every compiled instance has nx = 36
+  if (h->L.nx != 36) {
+    h->err = "internal: time-parallel element size";
+    return RBT_ERR_STATE;
+  }
+  if (!h->d_tp_elem) {
+    RBT_CUDA(h, cudaMalloc(&h->d_tp_elem, size_t(h->batch) * h->n_grid_max * esz * 8));
+    RBT_CUDA(h, cudaMalloc(&h->d_tp_fail, size_t(h->batch) * sizeof(int)));
+    RBT_CUDA(h, cudaMemset(h->d_tp_fail, 0, size_t(h->batch) * sizeof(int)));
+  }
+  if (S > h->tp_cap) {
+    for (int q = 0; q < 2; ++q) {
+      cudaFree(h->d_tp_scan[q]);
+      h->d_tp_scan[q] = nullptr;
+      RBT_CUDA(h, cudaMalloc(&h->d_tp_scan[q], size_t(h->batch) * (S + 1) * esz * 8));
+    }
+    cudaFree(h->d_tp_fmap);
+    cudaFree(h->d_tp_dx);
+    h->d_tp_fmap = h->d_tp_dx = nullptr;
+    RBT_CUDA(h, cudaMalloc(&h->d_tp_fmap, size_t(h->batch) * S * (h->L.nx * h->L.nx + h->L.nx) * 8));
+    RBT_CUDA(h, cudaMalloc(&h->d_tp_dx, size_t(h->batch) * S * h->L.nx * 8));
+    h->tp_cap = S;
+  }
+  return RBT_OK;
+}
+
+static rbt::TpParams tp_params(rbt_handle* h, int S) {
+  rbt::TpParams q{};
+  const int b0 = win_b0(h), nb = win_nb(h);
+  const size_t go = size_t(b0) * h->n_grid;
+  const size_t esz = rbt::TpElem<2 * 18>::SIZE;
+  q.L = h->L;
+  q.ctrl = h->d_ctrl;
+  q.n_grid = h->n_grid;
+  q.batch = nb;
+  q.segs = S;
+  q.kkt = h->d_kkt + go * h->L.k_stride;
+  q.ric = h->d_ric + go * h->L.r_stride;
+  q.elem = h->d_tp_elem + go * esz;
+  q.fmap = h->d_tp_fmap + size_t(b0) * S * (h->L.nx * h->L.nx + h->L.nx);
+  q.dxseed = h->d_tp_dx + size_t(b0) * S * h->L.nx;
+  q.dx0 = h->d_dx0 + size_t(b0) * h->L.nx;
+  q.fail = h->d_tp_fail + b0;
+  return q;
+}
+
+// Elements, in-segment reduction and suffix scan: returns (in h->tp_seeds) the scan buffer whose entry j + 1 is (P, s) at hi_j.
+template <int NV, int NU, int NS>
+static int tp_backward_boundaries(rbt_handle* h, int S, cudaStream_t st) {
+  constexpr int NX = 2 * NV;
+  using CC = rbt::TpCombCfg<NX>;
+  const size_t esz = rbt::TpElem<NX>::SIZE;
+  if (!h->attr_tp) {
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::tp_combine_kernel<NX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CC::SMEM_BYTES));
+    h->attr_tp = true;
+  }
+  const int b0 = win_b0(h), nb = win_nb(h), N = h->n_grid - 1;
+  rbt::TpParams q = tp_params(h, S);
+  RBT_CUDA(h, cudaMemsetAsync(h->d_tp_fail + b0, 0, size_t(nb) * sizeof(int), st));
+  rbt::tp_element_kernel<NV, NU, NS><<<nb * h->n_grid, rbt::TpElemCfg<NV, NU, NS>::NT, 0, st>>>(q);
+  h->launches += 1;
+  int lmax = 0;
+  for (int j = 0; j < S; ++j) lmax = std::max(lmax, rbt::tp_seg_lo(j + 1, N, S) - rbt::tp_seg_lo(j, N, S));
+  q.gather = -1;
+  for (int d = 1; d < lmax; d *= 2) {  // tree reduction inside every segment, in place
+    q.d = d;
+    q.pairs = (lmax + 2 * d - 1) / (2 * d);
+    rbt::tp_combine_kernel<NX><<<nb * S * q.pairs, CC::NT, CC::SMEM_BYTES, st>>>(q);
+    h->launches += 1;
+  }
+  int cur = 0;
+  q.gather = 1;
+  for (int d = 1; d < S + 1; d *= 2) {  // suffix scan over the aggregates and the terminal element
+    q.d = d;
+    q.scan_in = h->d_tp_scan[cur ^ 1] + size_t(b0) * (S + 1) * esz;
+    q.scan_out = h->d_tp_scan[cur] + size_t(b0) * (S + 1) * esz;
+    rbt::tp_combine_kernel<NX><<<nb * (S + 1), CC::NT, CC::SMEM_BYTES, st>>>(q);
+    h->launches += 1;
+    q.gather = 0;
+    cur ^= 1;
+  }
+  h->tp_seeds = h->d_tp_scan[cur ^ 1];
+  RBT_CUDA(h, cudaGetLastError());
+  return RBT_OK;
+}
+
 template <int NV, int NU, int NS>
 static int launch_backward(rbt_handle* h, int write_fact, cudaStream_t st) {
   constexpr int NP = 6;
@@ -510,11 +643,16 @@ static int launch_backward(rbt_handle* h, int write_fact, cudaStream_t st) {
     h->err = "internal: shared-memory staging size does not match rbt_layout";
     return RBT_ERR_STATE;
   }
-  auto kern_s = rbt::riccati_backward_kernel<NV, NU, NS, NP, true>;   // Fqq = I, Fqv = dt I outside the floating-base blocks
-  auto kern_g = rbt::riccati_backward_kernel<NV, NU, NS, NP, false>;  // any Fxx
+  const int S = tp_segments(h);
+  auto kern_s = S > 1 ? rbt::riccati_backward_kernel<NV, NU, NS, NP, true, true>   // Fqq = I, Fqv = dt I outside the floating-base blocks
+                      : rbt::riccati_backward_kernel<NV, NU, NS, NP, true>;
+  auto kern_g = S > 1 ? rbt::riccati_backward_kernel<NV, NU, NS, NP, false, true>  // any Fxx
+                      : rbt::riccati_backward_kernel<NV, NU, NS, NP, false>;
   if (!h->attr_bwd) {  // the attribute is per device: tracked per handle (a handle lives on one device)
-    RBT_CUDA(h, cudaFuncSetAttribute(kern_s, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
-    RBT_CUDA(h, cudaFuncSetAttribute(kern_g, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::riccati_backward_kernel<NV, NU, NS, NP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::riccati_backward_kernel<NV, NU, NS, NP, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::riccati_backward_kernel<NV, NU, NS, NP, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::riccati_backward_kernel<NV, NU, NS, NP, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
     h->attr_bwd = true;
   }
   rbt::BwdParams p;
@@ -534,6 +672,17 @@ static int launch_backward(rbt_handle* h, int write_fact, cudaStream_t st) {
   p.timeline = h->d_timeline;
   p.timeline_cta = h->timeline_cta;
   p.struct_flag = nullptr;
+  p.segs = S;
+  p.seeds = nullptr;
+  p.tp_fail = nullptr;
+  const int grid = nb * S;
+  if (S > 1) {
+    int rc = tp_ensure(h, S);
+    if (!rc) rc = tp_backward_boundaries<NV, NU, NS>(h, S, st);
+    if (rc) return rc;
+    p.seeds = h->tp_seeds + size_t(b0) * (S + 1) * rbt::TpElem<2 * NV>::SIZE;
+    p.tp_fail = h->d_tp_fail + b0;
+  }
   if (!h->keep_info) RBT_CUDA(h, cudaMemsetAsync(h->d_info + b0, 0, size_t(nb) * sizeof(int), st));
   h->keep_info = false;
   if (h->stagger_ns > 0) RBT_CUDA(h, cudaMemsetAsync(h->d_arrivals, 0, 1024 * sizeof(int), st));
@@ -543,17 +692,17 @@ static int launch_backward(rbt_handle* h, int write_fact, cudaStream_t st) {
   const bool known_struct = h->kkt_from_condense || h->fxx_mode == RBT_FXX_MECHANICAL;
   h->kkt_from_condense = false;
   if (known_struct) {
-    kern_s<<<nb, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
+    kern_s<<<grid, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
     h->launches += 1;
   } else if (h->fxx_mode == RBT_FXX_GENERAL) {
-    kern_g<<<nb, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
+    kern_g<<<grid, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
     h->launches += 1;
   } else {
     RBT_CUDA(h, cudaMemsetAsync(h->d_struct, 0, 2 * sizeof(int), st));
     rbt::check_fxx_structure_kernel<NV, NP><<<(nb * (h->n_grid - 1) + 7) / 8, 256, 0, st>>>(p, h->d_struct);
     p.struct_flag = h->d_struct;
-    kern_s<<<nb, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
-    kern_g<<<nb, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
+    kern_s<<<grid, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
+    kern_g<<<grid, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
     h->launches += 3;
   }
   RBT_CUDA(h, cudaGetLastError());
@@ -569,9 +718,12 @@ int rbt_set_fxx_structure(rbt_handle* h, int mode) {
 template <int NV, int NU, int NS>
 static int launch_forward(rbt_handle* h, cudaStream_t st) {
   using C = rbt::FwdCfg<NV, NU, NS>;
-  auto kern = rbt::riccati_forward_kernel<NV, NU, NS>;
+  const int S = tp_segments(h);
+  auto kern = S > 1 ? rbt::riccati_forward_kernel<NV, NU, NS, true> : rbt::riccati_forward_kernel<NV, NU, NS>;
   if (!h->attr_fwd) {
-    RBT_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::riccati_forward_kernel<NV, NU, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::riccati_forward_kernel<NV, NU, NS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    RBT_CUDA(h, cudaFuncSetAttribute(rbt::tp_fwd_compose_kernel<NV, NU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rbt::TpFwdCfg<NV, NU>::SMEM_BYTES));
     h->attr_fwd = true;
   }
   rbt::FwdParams p;
@@ -585,7 +737,20 @@ static int launch_forward(rbt_handle* h, cudaStream_t st) {
   p.ric = h->d_ric + go * h->L.r_stride;
   p.dx0 = h->d_dx0 + size_t(b0) * h->L.nx;
   p.dir = h->d_dir + go * h->L.d_stride;
-  kern<<<nb, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
+  p.segs = S;
+  p.dxseed = nullptr;
+  p.tp_fail = nullptr;
+  if (S > 1) {
+    // the backward sweep of this handle ran segmented too (same rule, same handle): its failure flags are current
+    if (int rc = tp_ensure(h, S)) return rc;
+    rbt::TpParams q = tp_params(h, S);
+    rbt::tp_fwd_compose_kernel<NV, NU><<<nb * (S - 1), rbt::TpFwdCfg<NV, NU>::NT, rbt::TpFwdCfg<NV, NU>::SMEM_BYTES, st>>>(q);
+    rbt::tp_fwd_boundary_kernel<2 * NV><<<nb, 64, 0, st>>>(q);
+    h->launches += 2;
+    p.dxseed = q.dxseed;
+    p.tp_fail = q.fail;
+  }
+  kern<<<nb * S, C::NTHREADS, C::SMEM_BYTES, st>>>(p);
   RBT_CUDA(h, cudaGetLastError());
   h->launches += 1;
   return RBT_OK;

@@ -84,6 +84,9 @@ __device__ __forceinline__ void l2_prefetch_bulk(const void* gmem_src, uint32_t 
 __host__ __device__ constexpr int tile_off(int t, int M) { return (8 * t + 8 <= M) ? 8 * t : (M >= 8 ? M - 8 : 0); }
 __host__ __device__ constexpr int num_tiles(int M) { return (M + 7) / 8; }
 
+// First grid point of segment j when the stages 0..N-1 are split into S contiguous segments (time-parallel sweeps).
+__host__ __device__ inline int tp_seg_lo(int j, int N, int S) { return (j * N) / S; }
+
 // One warp accumulates NT 8x8 tiles of one 8-row band:  acc[n] += sum_k A(i0+g, k) * B(k, joff(n)+g).
 //   fa(i, k) / fb(k, j) return the operand element (shared-memory loads).  K need not be a multiple of 4.
 // n_begin (warp-uniform): tiles n < n_begin are skipped (symmetric products: only the tiles on/above the diagonal band).

@@ -43,6 +43,17 @@ struct BwdParams {
   const int* struct_flag;  // device: 0 = every Fxx of the batch has the mechanical structure (nullptr: run unconditionally)
   long long* timeline;  // bring-up: [n_grid][2 roles][16] clock64 stamps of CTA `timeline_cta` (nullptr = off)
   int timeline_cta;
+  // time-parallel sweep (SEG instances only, riccati_time_parallel.cuh): CTA (ocp, j) of segs per OCP sweeps [lo_j, hi_j)
+  int segs;
+  const double* seeds;  // [batch][segs + 1][TpElem::SIZE]: entry j + 1 holds (P, s) at hi_j as (J, eta)
+  const int* tp_fail;   // [batch]: nonzero = an element factorisation failed, CTA (ocp, 0) sweeps the whole horizon
+};
+
+// A conditional value-function element (A, b, C, eta, J) of the time-parallel sweep, packed (A, C, J col-major nx x nx).
+template <int NX>
+struct TpElem {
+  static constexpr int A = 0, C = NX * NX, J = 2 * NX * NX, b = 3 * NX * NX, eta = 3 * NX * NX + NX, SIZE = 3 * NX * NX + 2 * NX;
+  static_assert(SIZE % 2 == 0, "16-byte aligned elements");
 };
 
 // NP = dim_passive (6: floating base, 0: fixed base).  STRUCT: the state-equation blocks have the structure every robotoc
@@ -148,7 +159,9 @@ __device__ __forceinline__ void chol_solve_smem(const double* Lm, const double* 
 #ifndef RBT_BWD_MIN_CTAS
 #define RBT_BWD_MIN_CTAS 4
 #endif
-template <int NV, int NU, int NS, int NP, bool STRUCT>
+// SEG: the time-parallel instance (riccati_time_parallel.cuh) -- CTA (ocp, j) sweeps segment j, seeded from p.seeds; a separate
+// instance, so the serial one keeps its register allocation.
+template <int NV, int NU, int NS, int NP, bool STRUCT, bool SEG = false>
 __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_CTAS) riccati_backward_kernel(const BwdParams p) {
   using C = BwdCfg<NV, NU, NS, NP>;
   constexpr int NX = C::NX, LDF = C::LDF, TX = C::TX, TU = C::TU, TV = C::TV, NTHR = C::NTHREADS, NG = C::NGEMM, KR = C::KR;
@@ -174,9 +187,19 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
   const rbt_layout& L = p.L;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
   const bool gemm_warp = warp < TX;
-  const int b = blockIdx.x;
+  const int b = SEG ? int(blockIdx.x) / p.segs : int(blockIdx.x);
   if (b >= p.batch) return;
   const int N = p.n_grid - 1;
+  int lo = 0, hi = N, seg = 0;  // this CTA sweeps grid points hi-1 .. lo
+  if constexpr (SEG) {
+    seg = int(blockIdx.x) % p.segs;
+    if (p.tp_fail[b] != 0) {
+      if (seg != 0) return;  // whole CTA: CTA (ocp, 0) sweeps the whole horizon from the terminal
+    } else {
+      lo = tp_seg_lo(seg, N, p.segs);
+      hi = tp_seg_lo(seg + 1, N, p.segs);
+    }
+  }
   // Records of grid point st of this OCP, formed from the kernel parameters where they are used: three 64-bit base pointers
   // held across the stage loop cost six registers, and the loop runs at the 80-register cap of 4 CTAs per SM.
   const int bst = b * p.n_grid;
@@ -269,10 +292,24 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
     }
   }
   __syncthreads();
-  if (tid == 0 && N > 0) issue_stage_load(N - 1);
+  if (tid == 0 && hi > lo) issue_stage_load(hi - 1);
 
+  bool seeded = false;
+  if constexpr (SEG) {
+    if (hi < N) {  // P, s at hi from the scan (a separate buffer: the CTA of the next segment writes the record at hi)
+      const double* sd = p.seeds + (size_t(b) * (p.segs + 1) + seg + 1) * TpElem<NX>::SIZE;
+      for (int e = tid; e < NX * NX; e += NTHR) sP[e] = sd[TpElem<NX>::J + e];
+      for (int e = tid; e < NX; e += NTHR) {
+        s_n[e] = sd[TpElem<NX>::eta + e];
+        Psin[e] = 0.0;
+        Phin[e] = 0.0;
+      }
+      if (tid < 8) scn[tid] = 0.0;
+      seeded = true;
+    }
+  }
   // ---- terminal stage: P_N = Qxx_N, s_N = -lx_N          riccati_recursion.cpp:37-38
-  {
+  if (!seeded) {
     const double* recN = kkt_at(N);
     double* ricN = ric_at(N);
     for (int e = tid; e < NX * NX; e += NTHR) {
@@ -293,7 +330,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
 
   uint32_t par0 = 0, par1 = 0;
 
-  for (int i = N - 1; i >= 0; --i) {
+  for (int i = hi - 1; i >= lo; --i) {
     const rbt_stage_ctrl cs = p.ctrl[i];
     const bool impact = (cs.type == RBT_IMPACT);
     const int ns = impact ? 0 : cs.ns;
@@ -591,7 +628,7 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
 
     // staging buffer is dead on plain stages: prefetch the next stage now (overlaps the rest of the stage)
     const bool early_prefetch = !extras;
-    if (early_prefetch && tid == 0 && i > 0) issue_stage_load(i - 1);
+    if (early_prefetch && tid == 0 && i > lo) issue_stage_load(i - 1);
 
     if (!impact) {
       if (sto) {
@@ -1000,14 +1037,14 @@ __global__ void __launch_bounds__(BwdCfg<NV, NU, NS, NP>::NTHREADS, RBT_BWD_MIN_
     RBT_TL(i, 13);
     __syncthreads();  // ---- barrier 5: P+ / s+ / STO state rolled
     RBT_TL(i, 14);
-    if (!early_prefetch && tid == 0 && i > 0) issue_stage_load(i - 1);
+    if (!early_prefetch && tid == 0 && i > lo) issue_stage_load(i - 1);
   }
 
   if (tid == 0) tma_store_wait_read();  // the last bulk store of P must have read shared memory before the CTA retires
   // ---- final phase transition at stage 0                       riccati_recursion.cpp:75-79
   {
     const rbt_stage_ctrl c0 = p.ctrl[0];
-    if (c0.sto && c0.sto_next && N > 0) {
+    if (c0.sto && c0.sto_next && N > 0 && lo == 0) {
       const double xi = scn[0], chi = scn[1], rho = scn[2], eta = scn[3], iota = scn[4];
       double sgm = xi - 2.0 * chi + rho;
       if ((sgm * p.max_dts0) < fabs(eta - iota) || sgm < 1.4901161193847656e-08) sgm = fabs(sgm) + fabs(eta - iota) / p.max_dts0;

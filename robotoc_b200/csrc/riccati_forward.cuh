@@ -22,6 +22,10 @@ struct FwdParams {
   const double* ric;
   const double* dx0;  // [batch][nx]
   double* dir;        // [batch][n_grid][d_stride]
+  // time-parallel sweep (SEG instance only, riccati_time_parallel.cuh)
+  int segs;
+  const double* dxseed;  // [batch][segs][nx]: dx at the first grid point of segment j >= 1
+  const int* tp_fail;    // [batch]: nonzero = CTA (ocp, 0) sweeps the whole horizon from dx0
 };
 
 template <int NV, int NU, int NS>
@@ -51,7 +55,9 @@ struct FwdCfg {
   static constexpr size_t SMEM_BYTES = size_t(SMEM_DOUBLES) * 8;
 };
 
-template <int NV, int NU, int NS>
+// SEG: the time-parallel instance -- CTA (ocp, j) sweeps grid points lo_j .. hi_j - 1 (the last segment through N) from
+// p.dxseed.  Ring slots and the dx ping-pong count from the segment's first grid point.
+template <int NV, int NU, int NS, bool SEG = false>
 __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forward_kernel(const FwdParams p) {
   using C = FwdCfg<NV, NU, NS>;
   constexpr int NX = C::NX, NTHR = C::NTHREADS;
@@ -60,9 +66,19 @@ __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forwa
   extern __shared__ __align__(16) double smem[];
   const rbt_layout& L = p.L;
   const int tid = threadIdx.x;
-  const int b = blockIdx.x;
+  const int b = SEG ? int(blockIdx.x) / p.segs : int(blockIdx.x);
   if (b >= p.batch) return;
   const int N = p.n_grid - 1;
+  int lo = 0, last = N, seg = 0;
+  if constexpr (SEG) {
+    seg = int(blockIdx.x) % p.segs;
+    if (p.tp_fail[b] != 0) {
+      if (seg != 0) return;
+    } else {
+      lo = tp_seg_lo(seg, N, p.segs);
+      last = (seg == p.segs - 1) ? N : tp_seg_lo(seg + 1, N, p.segs) - 1;
+    }
+  }
   const double* kkt_b = p.kkt + size_t(b) * p.n_grid * L.k_stride;
   const double* ric_b = p.ric + size_t(b) * p.n_grid * L.r_stride;
   double* dir_b = p.dir + size_t(b) * p.n_grid * L.d_stride;
@@ -81,7 +97,7 @@ __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forwa
   };
   // one elected thread: all copies of grid point st into ring slot st&1
   auto issue = [&](int st) {
-    const int slot = st & 1;
+    const int slot = (st - lo) & 1;
     double* base = smem + slot * C::SLOT;
     const rbt_stage_ctrl c = p.ctrl[st];
     const double* krec = kkt_b + size_t(st) * L.k_stride;
@@ -118,20 +134,20 @@ __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forwa
     for (int q = 0; q < 4; ++q) mbar_init(&bars[q], 1);
     fence_mbar_init();
   }
-  if (tid < NX) sdx[tid] = p.dx0[size_t(b) * NX + tid];
+  if (tid < NX) sdx[tid] = (SEG && lo > 0) ? p.dxseed[(size_t(b) * p.segs + seg) * NX + tid] : p.dx0[size_t(b) * NX + tid];
   if (tid == 0) {
     ssc[0] = 0.0;
     ssc[1] = 0.0;
   }
   __syncthreads();
   if (tid == 0) {
-    issue(0);
-    if (N >= 1) issue(1);
+    issue(lo);
+    if (last >= lo + 1) issue(lo + 1);
   }
   uint32_t pe0 = 0, pe1 = 0;  // extras-barrier parity per slot
 
-  for (int i = 0; i <= N; ++i) {
-    const int slot = i & 1;
+  for (int i = lo; i <= last; ++i) {
+    const int slot = (i - lo) & 1;
     const rbt_stage_ctrl c = p.ctrl[i];
     const double* base = smem + slot * C::SLOT;
     const double* sA = base;
@@ -142,8 +158,8 @@ __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forwa
     const double* sKt = ss + ((NX + 1) & ~1);
     const double* sk = sKt + ((NU * NX + 1) & ~1);
     const double* ex = base + C::KPART + C::RPART;
-    double* dx = sdx + (i & 1) * NX;
-    double* dxn = sdx + ((i + 1) & 1) * NX;
+    double* dx = sdx + ((i - lo) & 1) * NX;
+    double* dxn = sdx + ((i - lo + 1) & 1) * NX;
     double* drec = dir_b + size_t(i) * L.d_stride;
     const bool terminal = (i == N);
     const bool impact = (!terminal && c.type == RBT_IMPACT);
@@ -151,7 +167,7 @@ __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forwa
     const bool sto = !terminal && c.sto, sto_next = !terminal && c.sto_next;
     const bool extras = !terminal && has_extras(i);
 
-    mbar_wait(&bars[slot], uint32_t(i >> 1) & 1u);
+    mbar_wait(&bars[slot], uint32_t((i - lo) >> 1) & 1u);
     if (extras) {
       if (slot) {
         mbar_wait(&bars[3], pe1);
@@ -261,7 +277,7 @@ __global__ void __launch_bounds__(FwdCfg<NV, NU, NS>::NTHREADS, 3) riccati_forwa
     if (tid == 0) {
       ssc[0] = dts;
       ssc[1] = dtsn;
-      if (i + 2 <= N) issue(i + 2);
+      if (i + 2 <= last) issue(i + 2);
     }
     __syncthreads();
   }

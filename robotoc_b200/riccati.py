@@ -86,6 +86,12 @@ class RiccatiRecursion:
         _check(self._lib.rbt_set_schedule(self._h, ctrl, n, self._max_dts0), self._err, "RiccatiRecursion")
         self._ctrl, self.n_grid = ctrl, n
 
+    def setTimeSegments(self, segments: int):
+        """Time-parallel sweeps (rbt_set_time_segments): 0 = automatic (default), 1 = serial, k > 1 = k segments of the
+        horizon on separate CTAs.  Needs the schedule (setTimeDiscretization) first; k > 1 is refused on a schedule with
+        switching-time optimisation and beyond n_grid - 1."""
+        _check(self._lib.rbt_set_time_segments(self._h, int(segments)), self._err, "RiccatiRecursion")
+
     def backwardRiccatiRecursion(self, kkt=None, write_fact=False, stream=None):
         """riccati_recursion.cpp:32-80.  `kkt` (host, [batch, n_grid, k_stride]) is uploaded when given; otherwise the
         device-resident KKT buffer (rbt_dev_ptr) is used as is."""
