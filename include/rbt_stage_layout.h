@@ -186,6 +186,9 @@ typedef struct rbt_wire_seg { int lin_off, wire_off, rows, cols, ld, sym; } rbt_
      2: the diagonal of a rows x rows block (rows doubles on the wire) -> element (k,k), ld */
 typedef struct rbt_wire_zero { int lin_off, n; } rbt_wire_zero;   /* sections of the record the device zero-fills (first) */
 enum { RBT_COST_GENERAL = 0, RBT_COST_ROBOTOC = 1 };
+/* OR-ed into cost_structure: the device fills the inverse-dynamics rows (rbt_linearize_inverse_dynamics), so non-terminal wire
+ * records carry neither M nor the first nv rows of dIDCdqv and IDC -- only their nf contact rows */
+#define RBT_WIRE_DEVICE_ID 2
 #define RBT_WIRE_MAX_SEGS 20
 #define RBT_WIRE_MAX_ZERO 5
 typedef struct rbt_wire_layout {
@@ -217,8 +220,9 @@ static inline RBT_HD void rbt_wire_add_qxx_(const rbt_stage_layout* L, int cost_
 static inline RBT_HD void rbt_make_wire_layout(const rbt_stage_layout* L, const rbt_stage_ctrl* c, int with_sto, int cost_structure,
                                                rbt_wire_layout* W) {
   const int nv = L->nv, nx = L->nx, nf = c->nf, nvf = nv + nf;
-  const int dc = (cost_structure == RBT_COST_ROBOTOC);
+  const int dc = ((cost_structure & RBT_COST_ROBOTOC) != 0), did = ((cost_structure & RBT_WIRE_DEVICE_ID) != 0);
   int ci;
+  cost_structure &= RBT_COST_ROBOTOC;
   W->nseg = 0; W->nzero = 0; W->w_doubles = 0; W->ocp_off = 0;
   if (c->type == RBT_TERMINAL) {
     rbt_wire_add_qxx_(L, cost_structure, W);
@@ -226,10 +230,16 @@ static inline RBT_HD void rbt_make_wire_layout(const rbt_stage_layout* L, const 
     rbt_wire_add_(W, L->l_se3 + 36, 36, 1, 36, 0);
     return;
   }
-  rbt_wire_add_(W, L->l_M, nv, nv, nv, 1);
-  if (nf > 0) rbt_wire_add_(W, L->l_J, nf, nv, L->nfm, 0);
-  rbt_wire_add_(W, L->l_D, nvf, nx, L->nvf, 0);
-  rbt_wire_add_(W, L->l_IDC, nvf, 1, nvf, 0);
+  if (!did) {
+    rbt_wire_add_(W, L->l_M, nv, nv, nv, 1);
+    if (nf > 0) rbt_wire_add_(W, L->l_J, nf, nv, L->nfm, 0);
+    rbt_wire_add_(W, L->l_D, nvf, nx, L->nvf, 0);
+    rbt_wire_add_(W, L->l_IDC, nvf, 1, nvf, 0);
+  } else if (nf > 0) {  /* contact rows only: dCda, [dCdq | dCdv], C */
+    rbt_wire_add_(W, L->l_J, nf, nv, L->nfm, 0);
+    rbt_wire_add_(W, L->l_D + nv, nf, nx, L->nvf, 0);
+    rbt_wire_add_(W, L->l_IDC + nv, nf, 1, nf, 0);
+  }
   rbt_wire_add_(W, L->l_Qaa, nv, 1, nv, 0);
   if (dc) rbt_wire_zero_(W, L->l_Qff, L->nfm * L->nfm);
   if (nf > 0) rbt_wire_add_(W, L->l_Qff, nf, nf, L->nfm, dc ? 2 : 1);

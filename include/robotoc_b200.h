@@ -178,6 +178,48 @@ int rbt_set_slack_and_dual_positive(rbt_handle* h, void* stream);
  * Order: rbt_upload(LIN, CON, SOL) -> rbt_linearize_joint_limits -> rbt_eval_kkt / rbt_condense. */
 int rbt_set_joint_limits(rbt_handle* h, const double* bound_host);
 int rbt_linearize_joint_limits(rbt_handle* h, void* stream);
+
+/* Robot model of the inverse-dynamics linearisation (SURVEY.md 8f-1, first slice): what pinocchio::Model holds for a floating-base
+ * tree of revolute joints, in Pinocchio's depth-first joint order.  Body b is Pinocchio joint b + 1 (joint 0 is the universe):
+ * body 0 is the free-flyer root, bodies 1 .. n_bodies-1 are revolute joints.  All frames are Pinocchio's joint frames.
+ *   parent[b]            parent body (parent[0] = -1, else 0 <= parent[b] < b)               model.parents[b+1] - 1
+ *   axis[b]              unit rotation axis of a revolute joint in its own frame (body 0: unused)  JointModelRevolute(Unaligned) axis
+ *   placement[b]         joint frame in the parent joint frame: R (column-major 3x3) | p     model.jointPlacements[b+1]
+ *   mass, com, inertia   Inertia of the body with the children of fixed joints merged in, rotational inertia about the centre of
+ *                        mass (column-major 3x3, symmetric positive definite)               model.inertias[b+1]
+ *   contact_parent[c], contact_placement[c]   parent body and placement jXf of point contact c    PointContact (point_contact.cpp)
+ *   gravity              model.gravity.linear()
+ * n_bodies = nv - 5 (six free-flyer velocities + one per revolute joint). */
+#define RBT_MAX_BODIES 32
+typedef struct rbt_robot_model {
+  int nv, n_bodies, n_contacts, pad_;
+  int parent[RBT_MAX_BODIES];
+  double axis[RBT_MAX_BODIES][3];
+  double placement[RBT_MAX_BODIES][12];
+  double mass[RBT_MAX_BODIES];
+  double com[RBT_MAX_BODIES][3];
+  double inertia[RBT_MAX_BODIES][9];
+  int contact_parent[RBT_MAX_CONTACTS];
+  double contact_placement[RBT_MAX_CONTACTS][12];
+  double gravity[3];
+} rbt_robot_model;
+/* Copies the model to the device; call once after rbt_stage_setup.  RBT_ERR_ARG if nv or n_contacts disagree with the handle,
+ * a parent is not earlier in the order, a mass is not positive, an inertia is not symmetric positive definite or an axis is not
+ * a unit vector (rbt_last_error names the entry). */
+int rbt_set_robot_model(rbt_handle* h, const rbt_robot_model* model);
+/* The inverse-dynamics rows of linearizeContactDynamics (src/dynamics/contact_dynamics.cpp:22-44: Robot::setContactForces, RNEA,
+ * RNEADerivatives, robot.hxx:494-580, fext[parent] = jXf.act(Force(f, 0)) per active point contact, point_contact.cpp:55-60) on
+ * Intermediate and Lift grid points and of linearizeImpactDynamics (impact_dynamics.cpp:17-35: RNEAImpact /
+ * RNEAImpactDerivatives, robot.hxx:589-622 -- v = 0, dv for a, the impulse as external force, no gravity) on Impact grid points,
+ * from q, v, a | dv, f, beta of RBT_BUF_SOL.  Writes into RBT_BUF_LIN: the nv ID rows of IDC (RNEA - [0; u]; impact: RNEA),
+ * the ID rows [dIDdq | dIDdv] of dIDCdqv (impact: [dIDdq | 0]), M = dIDda (impact: dIDddv), symmetrised from its upper
+ * triangle like Robot::RNEADerivatives, and adds lq += dIDdq^T beta, lv += dIDdv^T beta, la (impact: ldv) += M^T beta
+ * (contact_dynamics.cpp:31-33, impact_dynamics.cpp:24-25).  Derivatives in q are taken in the tangent space, q (+) dq =
+ * integrate(q, dq) with the free flyer as [p | quaternion xyzw] and the local SE(3) exponential.  Terminal grid points are
+ * untouched.  Order: rbt_upload(LIN, CON, SOL) -> (rbt_linearize_joint_limits) -> rbt_linearize_inverse_dynamics ->
+ * rbt_eval_kkt / rbt_condense; the uploaded records' ID sections are ignored and their gradients lack the beta terms.
+ * RBT_ERR_STATE before rbt_set_robot_model. */
+int rbt_linearize_inverse_dynamics(rbt_handle* h, void* stream);
 /* computeInitialStateDirection (src/dynamics/state_equation.cpp:98-109) into RBT_BUF_DX0.  dq0_v0_host: [batch][2 nv] =
  * {q0 (-) s[0].q from Robot::subtractConfiguration (the robot model stays on the host), v0}; uses the stage-0 Fqq_prev_inv that
  * rbt_condense left in RBT_BUF_EXP and s[0].v of RBT_BUF_SOL, so call it after rbt_condense and before rbt_riccati_forward. */
@@ -248,7 +290,11 @@ int rbt_iteration_host_resident(rbt_handle* h, const double* wire_host, const do
  * cost Hessians the way every cost component robotoc ships produces them -- Qqq dense, Qvv / Quu / Qff diagonal, Qqv = 0
  * (configuration_space_cost.cpp:308-322, task_space_*_cost.cpp, com_cost.cpp, local_contact_force_cost.cpp:130) -- 23 % fewer
  * bytes again; a problem with user-defined cost components that fill other entries uses RBT_COST_GENERAL (default).
- * rbt_set_wire_cost_structure tells the handle which of the two the host's wire records are in. */
+ * rbt_set_wire_cost_structure tells the handle which of the two the host's wire records are in.
+ * RBT_WIRE_DEVICE_ID OR-ed into cost_structure (rbt_stage_layout.h): the device computes the inverse-dynamics rows
+ * (rbt_linearize_inverse_dynamics, after rbt_set_robot_model), so the wire records drop M, the ID rows of dIDCdqv and of IDC,
+ * and their gradients lack the beta terms; rbt_iteration_host_wire / _resident run the kernel right after the unpack and
+ * rbt_iteration_host_bytes counts the smaller records. */
 int rbt_set_wire_cost_structure(rbt_handle* h, int cost_structure);
 int rbt_wire_doubles(const rbt_stage_dims* sdims, const rbt_stage_ctrl* ctrl, int n_grid, int cost_structure);   /* doubles per OCP */
 int rbt_wire_layout_get(const rbt_stage_dims* sdims, const rbt_stage_ctrl* ctrl, int n_grid, int cost_structure, int i,

@@ -411,9 +411,24 @@ class DirectMultipleShooting {
     if (dq0_v0.size() != size_t(rr_.batch()) * 2 * S_.nv) throw std::invalid_argument("[DirectMultipleShooting] invalid argument: size of 'dq0_v0'");
     rr_.check(rbt_initial_state_direction(rr_.handle(), dq0_v0.data(), nullptr));
   }
+  /// The robot model of the inverse-dynamics linearisation (rbt_robot_model, filled from pinocchio::Model; INTEGRATION.md 5b).
+  void setRobotModel(const rbt_robot_model& model) { rr_.check(rbt_set_robot_model(rr_.handle(), &model)); }
+  /// The inverse-dynamics rows of linearizeContactDynamics / linearizeImpactDynamics on the device (rbt_linearize_inverse_dynamics):
+  /// `lin` (records without the ID rows and without the beta terms of the gradients) and `sol` are uploaded, `lin` is read back
+  /// with IDC / dIDCdqv ID rows, M and the beta terms filled in.
+  void linearizeInverseDynamics(std::vector<double>& lin, const std::vector<double>& sol) {
+    expect(lin, S_.l_stride, "lin");
+    expect(sol, S_.s_stride, "sol");
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_SOL, sol.data(), nullptr));
+    rr_.check(rbt_linearize_inverse_dynamics(rr_.handle(), nullptr));
+    rr_.check(rbt_download(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
+    rr_.check(rbt_sync(rr_.handle(), nullptr));
+  }
   /// Host wire records of the schedule in force (rbt_stage_layout.h): what an adaptor sends instead of the dense records.
-  void setWireCostStructure(bool robotoc_costs) {
-    cost_structure_ = robotoc_costs ? RBT_COST_ROBOTOC : RBT_COST_GENERAL;
+  /// device_inverse_dynamics: the records leave M and the ID rows of dIDCdqv / IDC to the device (RBT_WIRE_DEVICE_ID).
+  void setWireCostStructure(bool robotoc_costs, bool device_inverse_dynamics = false) {
+    cost_structure_ = (robotoc_costs ? RBT_COST_ROBOTOC : RBT_COST_GENERAL) | (device_inverse_dynamics ? RBT_WIRE_DEVICE_ID : 0);
     rr_.check(rbt_set_wire_cost_structure(rr_.handle(), cost_structure_));
   }
   std::vector<double> packWire(const std::vector<double>& lin, const std::vector<rbt_stage_ctrl>& ctrl) const {

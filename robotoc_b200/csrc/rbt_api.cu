@@ -1,5 +1,6 @@
 // rbt_api.cu -- C ABI of librobotoc_b200.so (see include/robotoc_b200.h for the reference interfaces replaced).
 // Plumbing only: handles, device buffers, stream-ordered copies and kernel launches.  No CPU compute path.
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <cstdint>
@@ -22,6 +23,7 @@
 #include "ustage_kernels.cuh"
 #include "eval_kernels.cuh"
 #include "line_search_kernels.cuh"
+#include "rnea_kernels.cuh"
 
 namespace {
 
@@ -90,6 +92,7 @@ struct rbt_handle {
   double* d_wire = nullptr;  // packed host wire records (rbt_iteration_host_wire), allocated on first use
   int* d_tgt = nullptr;           // box rows per PDIPM target (stage_kernels.cuh: StageParams::tgt)
   double* d_bound = nullptr;      // joint limits per box row (rbt_set_joint_limits)
+  rbt::RneaModel* d_model = nullptr;  // robot model of rbt_linearize_inverse_dynamics (rbt_set_robot_model)
   double* d_res_stage = nullptr;  // rbt_iteration_host_resident: compact residuals in, compact slack|dual out
   double* d_sd_stage = nullptr;
   std::vector<rbt_wire_layout> Wv;   // per grid point (the wire record of a grid point depends on its control word)
@@ -224,6 +227,7 @@ int rbt_destroy(rbt_handle* h) {
     cudaFree(h->d_W);
     cudaFree(h->d_tgt);
     cudaFree(h->d_bound);
+    cudaFree(h->d_model);
     cudaFree(h->d_res_stage);
     cudaFree(h->d_sd_stage);
     if (h->s_h2d) cudaStreamDestroy(h->s_h2d);
@@ -1043,6 +1047,77 @@ int rbt_linearize_joint_limits(rbt_handle* h, void* stream) {
   return RBT_OK;
 }
 
+int rbt_set_robot_model(rbt_handle* h, const rbt_robot_model* m) {
+  if (!h || !m) return RBT_ERR_ARG;
+  if (!h->stage_ready) {
+    h->err = "[rbt_set_robot_model] stage layer not set up";
+    return RBT_ERR_STATE;
+  }
+  auto bad = [&](const std::string& what) {
+    h->err = "[rbt_set_robot_model] invalid argument: " + what;
+    return RBT_ERR_ARG;
+  };
+  if (m->nv != h->S.nv || m->n_bodies != m->nv - 5 || m->n_bodies > RBT_MAX_BODIES) return bad("nv / n_bodies disagree with the handle");
+  if (m->n_contacts != h->S.ncon) return bad("n_contacts disagrees with the stage layer");
+  rbt::RneaModel d = {};
+  d.nb = m->n_bodies;
+  d.ncon = m->n_contacts;
+  for (int b = 0; b < m->n_bodies; ++b) {
+    const std::string tag = "body " + std::to_string(b) + ": ";
+    if (b == 0 ? m->parent[b] != -1 : (m->parent[b] < 0 || m->parent[b] >= b)) return bad(tag + "parent must come earlier in the order");
+    if (!(m->mass[b] > 0.0)) return bad(tag + "mass must be positive");
+    const double* I = m->inertia[b];
+    double imax = 0.0;
+    for (int e = 0; e < 9; ++e) imax = std::max(imax, std::fabs(I[e]));
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < i; ++j)
+        if (!(std::fabs(I[i + 3 * j] - I[j + 3 * i]) <= 1e-12 * imax)) return bad(tag + "inertia is not symmetric");
+    // Sylvester: leading minors of a symmetric 3x3
+    const double m1 = I[0], m2 = I[0] * I[4] - I[1] * I[3];
+    const double m3 = I[0] * (I[4] * I[8] - I[5] * I[7]) - I[3] * (I[1] * I[8] - I[2] * I[7]) + I[6] * (I[1] * I[5] - I[2] * I[4]);
+    if (!(m1 > 0.0 && m2 > 0.0 && m3 > 0.0)) return bad(tag + "inertia is not positive definite");
+    if (b > 0) {
+      const double* u = m->axis[b];
+      if (!(std::fabs(std::sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]) - 1.0) <= 1e-12)) return bad(tag + "axis is not a unit vector");
+    }
+    d.parent[b] = m->parent[b];
+    for (int e = 0; e < 3; ++e) {
+      d.axis[b][e] = m->axis[b][e];
+      d.p[b][e] = m->placement[b][9 + e];
+      d.com[b][e] = m->com[b][e];
+    }
+    for (int e = 0; e < 9; ++e) {
+      d.R[b][e] = m->placement[b][e];
+      d.Ic[b][e] = I[e];
+    }
+    d.mass[b] = m->mass[b];
+  }
+  for (int c = 0; c < m->n_contacts; ++c) {
+    if (m->contact_parent[c] < 0 || m->contact_parent[c] >= m->n_bodies) return bad("contact " + std::to_string(c) + ": no such parent body");
+    d.cparent[c] = m->contact_parent[c];
+    for (int e = 0; e < 9; ++e) d.cR[c][e] = m->contact_placement[c][e];
+    for (int e = 0; e < 3; ++e) d.cp[c][e] = m->contact_placement[c][9 + e];
+  }
+  for (int e = 0; e < 3; ++e) d.gravity[e] = m->gravity[e];
+  RBT_CUDA(h, cudaSetDevice(h->device));
+  if (!h->d_model) RBT_CUDA(h, cudaMalloc(&h->d_model, sizeof(rbt::RneaModel)));
+  RBT_CUDA(h, cudaMemcpy(h->d_model, &d, sizeof(rbt::RneaModel), cudaMemcpyHostToDevice));
+  return RBT_OK;
+}
+
+int rbt_linearize_inverse_dynamics(rbt_handle* h, void* stream) {
+  RBT_STAGE_CHECK(h, "rbt_linearize_inverse_dynamics");
+  if (!h->d_model) {
+    h->err = "[rbt_linearize_inverse_dynamics] call rbt_set_robot_model first";
+    return RBT_ERR_STATE;
+  }
+  rbt::linearize_inverse_dynamics_kernel<18><<<win_nb(h) * h->n_grid, rbt::RneaCfg<18>::NTHR, 0, (cudaStream_t)stream>>>(
+      make_stage_params(h), h->d_model);
+  RBT_CUDA(h, cudaGetLastError());
+  h->launches += 1;
+  return RBT_OK;
+}
+
 int rbt_initial_state_direction(rbt_handle* h, const double* dq0_v0_host, void* stream) {
   RBT_STAGE_CHECK(h, "rbt_initial_state_direction");
   if (!dq0_v0_host) return RBT_ERR_ARG;
@@ -1252,6 +1327,10 @@ static int iteration_host_impl(rbt_handle* h, const double* wire_host, const dou
     if (rcw != RBT_OK) return rcw;
     bool sw = false;
     for (int i = 0; i < h->n_grid; ++i) sw = sw || (h->ctrl[i].ns > 0 && h->ctrl[i].type != RBT_IMPACT);
+    if ((h->cost_structure & RBT_WIRE_DEVICE_ID) && !h->d_model) {
+      h->err = "[rbt_iteration_host_wire] the wire records leave the inverse dynamics to the device: call rbt_set_robot_model first";
+      return RBT_ERR_STATE;
+    }
     if (sw && !lin_host) {
       h->err = "[rbt_iteration_host_wire] invalid argument: the schedule has switching-constraint stages, their sections come from lin_host_switching";
       return RBT_ERR_ARG;
@@ -1320,6 +1399,7 @@ static int iteration_host_impl(rbt_handle* h, const double* wire_host, const dou
       wp.c_stride = h->S.c_stride; wp.c_res = h->S.c_res; wp.ncp = h->S.ncp;
       rbt::unpack_wire_kernel<<<nb * h->n_grid, 128, 0, st>>>(wp);
       h->launches += 1;
+      if ((h->cost_structure & RBT_WIRE_DEVICE_ID) && (rc = rbt_linearize_inverse_dynamics(h, stream)) != RBT_OK) break;
     }
     if (!(rc = rbt_condense(h, stream)) && !(rc = rbt_riccati_backward(h, 0, stream)) && !(rc = rbt_riccati_forward(h, stream)) &&
         !(rc = rbt_expand_and_step_sizes(h, stream)))
@@ -1371,7 +1451,7 @@ int rbt_iteration_host_resident(rbt_handle* h, const double* wire_host, const do
 }
 
 int rbt_set_wire_cost_structure(rbt_handle* h, int cost_structure) {
-  if (!h || (cost_structure != RBT_COST_GENERAL && cost_structure != RBT_COST_ROBOTOC)) return RBT_ERR_ARG;
+  if (!h || (cost_structure & ~(RBT_COST_ROBOTOC | RBT_WIRE_DEVICE_ID)) != 0) return RBT_ERR_ARG;
   if (h->cost_structure != cost_structure) h->wire_dirty = true;
   h->cost_structure = cost_structure;
   return RBT_OK;

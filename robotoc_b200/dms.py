@@ -17,6 +17,18 @@ from .riccati import RiccatiRecursion, _check, _vp
 from .stage import StageDims, StageLayout
 
 LIN, CON, EXP, SOL, XDIR, STEPS, PERF = 6, 7, 8, 9, 10, 11, 12
+RBT_MAX_BODIES, RBT_MAX_CONTACTS = 32, 8
+WIRE_DEVICE_ID = 2  # RBT_WIRE_DEVICE_ID (rbt_stage_layout.h)
+
+
+class rbt_robot_model(ctypes.Structure):
+    """include/robotoc_b200.h: floating-base tree of revolute joints in Pinocchio's joint order (body b = Pinocchio joint b+1)."""
+    _fields_ = [("nv", ctypes.c_int), ("n_bodies", ctypes.c_int), ("n_contacts", ctypes.c_int), ("pad_", ctypes.c_int),
+                ("parent", ctypes.c_int * RBT_MAX_BODIES), ("axis", (ctypes.c_double * 3) * RBT_MAX_BODIES),
+                ("placement", (ctypes.c_double * 12) * RBT_MAX_BODIES), ("mass", ctypes.c_double * RBT_MAX_BODIES),
+                ("com", (ctypes.c_double * 3) * RBT_MAX_BODIES), ("inertia", (ctypes.c_double * 9) * RBT_MAX_BODIES),
+                ("contact_parent", ctypes.c_int * RBT_MAX_CONTACTS),
+                ("contact_placement", (ctypes.c_double * 12) * RBT_MAX_CONTACTS), ("gravity", ctypes.c_double * 3)]
 
 
 class DirectMultipleShooting:
@@ -71,6 +83,17 @@ class DirectMultipleShooting:
         """The joint-limit half of Constraints::linearizeConstraints on the device (rbt_linearize_joint_limits): PDIPM residuals
         of the box rows from the resident solution, and their dual terms added to the gradients of the linearization records."""
         _check(self._lib.rbt_linearize_joint_limits(self._h, stream), self.rr._err, "DirectMultipleShooting")
+
+    def setRobotModel(self, model: rbt_robot_model):
+        """Copies the robot model (rbt_robot_model: what pinocchio::Model holds for the tree) to the device, for
+        linearizeInverseDynamics and the device-side inverse dynamics of the wire paths."""
+        _check(self._lib.rbt_set_robot_model(self._h, ctypes.byref(model)), self.rr._err, "DirectMultipleShooting")
+
+    def linearizeInverseDynamics(self, stream=None):
+        """The inverse-dynamics rows of linearizeContactDynamics / linearizeImpactDynamics on the device
+        (rbt_linearize_inverse_dynamics): IDC and dIDCdqv ID rows, M, and the beta terms of lq, lv, la | ldv, from the resident
+        solution records."""
+        _check(self._lib.rbt_linearize_inverse_dynamics(self._h, stream), self.rr._err, "DirectMultipleShooting")
 
     def computeStepSizes(self, stream=None):
         _check(self._lib.rbt_expand_and_step_sizes(self._h, stream), self.rr._err, "DirectMultipleShooting")
@@ -144,10 +167,12 @@ class DirectMultipleShooting:
                self.rr._err, "DirectMultipleShooting")
         return h2d.value, d2h.value
 
-    def setWireCostStructure(self, robotoc_costs: bool):
+    def setWireCostStructure(self, robotoc_costs: bool, device_inverse_dynamics: bool = False):
         """Which cost-Hessian structure the host's wire records have: False = general (full packed triangles of Qxx, Quu, Qff),
-        True = what robotoc's shipped cost components produce (Qqq dense, Qvv / Quu / Qff diagonal, Qqv = 0)."""
-        self._cost_structure = 1 if robotoc_costs else 0
+        True = what robotoc's shipped cost components produce (Qqq dense, Qvv / Quu / Qff diagonal, Qqv = 0).
+        device_inverse_dynamics: the wire records leave out M and the ID rows of dIDCdqv and IDC (and their gradients the beta
+        terms); iteration_host_wire / iteration_host_resident compute them on the device (setRobotModel first)."""
+        self._cost_structure = (1 if robotoc_costs else 0) | (WIRE_DEVICE_ID if device_inverse_dynamics else 0)
         _check(self._lib.rbt_set_wire_cost_structure(self._h, self._cost_structure), self.rr._err, "DirectMultipleShooting")
 
     def pack_wire(self, lin):
