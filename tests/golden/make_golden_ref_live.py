@@ -1,11 +1,13 @@
-"""Generates tests/golden/golden_ref_live.npz and tests/golden/golden_ref_gaits.npz: the reference's own outputs
+"""Generates tests/golden/golden_ref_live.npz, golden_ref_gaits.npz and golden_ref_horizon.npz: the reference's own outputs
 (oracle/_ref/libref_riccati.so, the robotoc sources compiled unmodified by oracle/Makefile.ref) for the cases on which tests/ compare the oracle with the reference code, so that
 those comparisons run everywhere without a robotoc checkout.  Only runs where one exists:
 
-    ROBOTOC_REFERENCE=<robotoc source tree> python tests/golden/make_golden_ref_live.py [live] [gaits]
+    ROBOTOC_REFERENCE=<robotoc source tree> python tests/golden/make_golden_ref_live.py [live] [gaits] [horizon]
 
 golden_ref_gaits.npz holds the cases on the crawl and contact-mask-walk schedules (odd contact counts, single-foot impacts,
-every contact mask); golden_ref_live.npz everything else.  Without arguments both files are written.
+every contact mask); golden_ref_horizon.npz the receding-horizon edge schedules (helpers.receding_horizon_schedules: t0 != 0,
+events on grid 1 and beside it, at the end of the horizon, tiny steps), sampled on the grid points next to t0, the events and
+the terminal; golden_ref_live.npz everything else.  Without arguments all three files are written.
 
 Large records are stored as a fixed, seeded sample of every section of every record (golden_sample.py); small outputs are
 stored whole.
@@ -23,10 +25,12 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, HERE)
 
 from golden_sample import groups, layout_bounds, load, put, restore  # noqa: E402,F401  (load, restore: used by the tests)
-from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, small_event_schedule, trot_schedule  # noqa: E402,E501
+from helpers import (RH_SETS, contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, receding_horizon_schedules,  # noqa: E402
+                     small_event_schedule, trot_schedule)
 
 PATH = os.path.join(HERE, "golden_ref_live.npz")
 GAITS_PATH = os.path.join(HERE, "golden_ref_gaits.npz")
+HORIZON_PATH = os.path.join(HERE, "golden_ref_horizon.npz")
 RIC_FIELDS = "r_P r_s r_K r_k r_M r_m r_Psi r_Phi r_T r_W r_psix r_psiu r_phix r_phiu r_mt r_mtn r_sc r_dtsdx r_stosc".split()
 STAGE_KEYS = ("kkt", "cc_cond", "ric", "d", "cc_exp", "xd_exp", "steps", "d_upd", "xd_upd", "cc_upd", "ex_upd")
 
@@ -55,6 +59,44 @@ def schedule(case):
 def fixture_path(case):
     """The fixture file that holds the reference's outputs of a case."""
     return GAITS_PATH if case in GAIT_CASES else PATH
+
+
+# receding-horizon edge cases: the edge schedules of the first two events of each gait cycle (a lift and an impact; every
+# placement of _edge_offsets), ImpactFrictionCone on every other one
+HORIZON_EVENTS = 2
+
+
+def horizon_cases():
+    """[(name, gait, sto, t0, ctrl, impact_cones, seed)] of golden_ref_horizon.npz."""
+    out = []
+    for g, sto in RH_SETS:
+        sched = receding_horizon_schedules(g, sto, "edge")
+        per_event = len(sched) // (4 if g == "trot" else 6)
+        for k, (t0, td, ev, ctrl) in enumerate(sched[:HORIZON_EVENTS * per_event]):
+            out.append((f"{g}{'_sto' if sto else ''}_{k}", g, sto, t0, td, ctrl, k % 2 == 1, 500 + len(out)))
+    return out
+
+
+def horizon_case(case, S_getter=None, K_getter=None):
+    """Inputs of one horizon case (batch 1)."""
+    from robotoc_b200 import ANYMAL, Layout, StageDims, StageLayout, anymal_constraint_table
+    from synth import make_stage_inputs
+    name, g, sto, t0, td, ctrl, icone, seed = case
+    table = anymal_constraint_table(impact_friction_cone=icone)
+    sd = StageDims(ANYMAL, nf_max=12, n_contacts=table.n_contacts, n_box=table.n_box)
+    S, K = StageLayout(sd, getter=S_getter), Layout(ANYMAL, getter=K_getter)
+    lin, con, sol, dx0 = make_stage_inputs(sd, S, ctrl, 1, seed, impact_cones=icone)
+    return table, sd, S, K, ctrl, lin, con, sol, dx0, icone
+
+
+def horizon_grids(ctrl):
+    """The grid points a horizon case stores: the first three, the last four, and each event's grid with its neighbours."""
+    n = len(ctrl)
+    keep = {0, 1, 2, n - 4, n - 3, n - 2, n - 1}
+    for i, c in enumerate(ctrl):
+        if c.type in (1, 2):
+            keep |= {i - 2, i - 1, i, i + 1}
+    return sorted(i for i in keep if 0 <= i < n)
 
 
 def joint_limit_problem(sched, batch, seed):
@@ -114,7 +156,7 @@ def filter_rounds(case_rng):
     return amax, cost, viol, cost[:, 0] + 0.1, viol[:, 0] + 0.01
 
 
-def main(outputs=("live", "gaits")):
+def main(outputs=("live", "gaits", "horizon")):
     import oracle_lib
     import ref_lib
     import make_golden_ref_stage as mgs
@@ -147,6 +189,25 @@ def main(outputs=("live", "gaits")):
         ref = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
         for k in STAGE_KEYS:
             put(files[fixture_path(case)], f"stage_{case}_{k}", ref[k], mgs.stage_groups(ref[k], k, S, K), seed, k_min=3, k_z=1)
+    files[HORIZON_PATH] = {}
+    for case in horizon_cases():
+        table, sd, S, K, ctrl, lin, con, sol, dx0, icone = horizon_case(case, lib.orc_stage_layout_get, lib.orc_layout_get)
+        ref = ref_lib.reference_iteration(sd, S, K, table, ctrl, lin, con, dx0)
+        keep = np.zeros(len(ctrl), dtype=bool)
+        keep[horizon_grids(ctrl)] = True
+        for k in STAGE_KEYS:
+            a = ref[k]
+            grp = mgs.stage_groups(a, k, S, K)
+            n_grp = int(grp.max()) + 1
+            if a.ndim == 3:  # records of the kept grid points only: one nonzero entry of every section
+                gids, first = np.unique(grp.reshape(-1), return_index=True)
+                on = [False] * n_grp
+                for gid, pos in zip(gids, first):
+                    on[gid] = bool(keep[(pos // a.shape[-1]) % len(ctrl)])
+                put(files[HORIZON_PATH], f"h_{case[0]}_{k}", a, grp, case[7], k_min=tuple(1 if o else 0 for o in on),
+                    k_z=tuple(0 for o in on))
+            else:
+                files[HORIZON_PATH][f"h_{case[0]}_{k}"] = a
     for icone in (False, True):
         table, sd, S, K, ctrl, lin, con, sol, dx0 = mgs.problem(lib.orc_stage_layout_get, lib.orc_layout_get, icone)
         table, ctrl, lin, con, dx0 = perf_case(sd, S, icone)
@@ -179,10 +240,10 @@ def main(outputs=("live", "gaits")):
         put(out, f"jl_{which}_lin", l_r, np.where(l_r != lin, 0, 1), 7, frac=(1.0, 0.0), k_min=(0, 256), k_z=(l_r.size, 32))
         put(out, f"jl_{which}_con", c_r, np.where(c_r != con, 0, 1), 8, frac=(1.0, 0.0), k_min=(0, 256), k_z=(c_r.size, 32))
     for path, data in files.items():
-        if {PATH: "live", GAITS_PATH: "gaits"}[path] in outputs:
+        if {PATH: "live", GAITS_PATH: "gaits", HORIZON_PATH: "horizon"}[path] in outputs:
             np.savez_compressed(path, **data)
             print("wrote", path, os.path.getsize(path) // 1024, "KiB;", ref.ref_version().decode())
 
 
 if __name__ == "__main__":
-    main(sys.argv[1:] or ("live", "gaits"))
+    main(sys.argv[1:] or ("live", "gaits", "horizon"))

@@ -67,6 +67,94 @@ def contact_mask_walk_schedule(dt=0.02):
     return td, ev, ctrl
 
 
+def _events_in_order(ev):
+    """The events of `ev` in time order: (time, is_impact, post_dimf, impact_dimf, post_mask, impact_mask, sto)."""
+    out = [(t, True, k, s) for k, (t, s) in enumerate(zip(ev.impact_times, ev.sto_impact))]
+    out += [(t, False, k, s) for k, (t, s) in enumerate(zip(ev.lift_times, ev.sto_lift))]
+    out.sort()
+    return [(t, imp, ev.phase_dimf[p + 1], ev.impact_dimf[k] if imp else 0, ev.phase_mask[p + 1], ev.impact_mask[k] if imp else 0, s)
+            for p, (t, imp, k, s) in enumerate(out)]
+
+
+def _cycles(one, period, n, sto):
+    """`n` copies of the one-cycle event list `one` (which ends in the contact set it starts from), copy k shifted by
+    k * period; every event's STO flag set to `sto`."""
+    ev = ContactEvents(phase_dimf=[one.phase_dimf[0]], phase_mask=[one.phase_mask[0]])
+    for k in range(n):
+        for t, imp, dimf, idimf, mask, imask, _ in _events_in_order(one):
+            ev.push_back(imp, k * period + t, dimf, impact_dimf=idimf, sto=sto, post_mask=mask, impact_mask=imask)
+    return ev
+
+
+# receding-horizon gaits: (one-cycle events, cycle period, T, N); the trot of anymal_trot_events repeats every 1.08 s, the
+# crawl of anymal_crawl_events every 2.08 s (the next cycle starts 0.04 s after the last impact, like the first one)
+RH_GAITS = {"trot": (anymal_trot_events, 1.08, 1.12, 40), "crawl": (anymal_crawl_events, 2.08, 2.16, 54)}
+
+
+def trot_cycles(n, sto=False):
+    return _cycles(anymal_trot_events(), RH_GAITS["trot"][1], n, sto)
+
+
+def crawl_cycles(n, sto=False):
+    return _cycles(anymal_crawl_events(), RH_GAITS["crawl"][1], n, sto)
+
+
+def _edge_offsets(dt, T):
+    """Where edge_t0s puts an event relative to t0: a hair after t0 (tiny first step), exactly on grid 1, 1e-9 either side
+    of it (inside the _EPS test of discretize), 2 * _EPS either side of it (outside that test), just inside and just outside
+    the last-interval margin, and exactly at t0 (excluded: grid 0 starts in the event's post-phase)."""
+    e = 2.0 * 1.4901161193847656e-08
+    return (1e-6 * dt, dt, dt - 1e-9, dt + 1e-9, dt - e, dt + e, T - 0.5 * dt - 1e-9, T - 0.5 * dt + 1e-9, 0.0)
+
+
+def receding_horizon_schedules(gait, sto, which, per_dt=4):
+    """The schedules an MPC loop meets while the horizon slides over gait `gait` ("trot" | "crawl", every event STO-enabled
+    iff `sto`), discretized like OCPSolver::discretize at each t0: `which` = "sweep" (t0 over one gait cycle in steps of
+    dt / per_dt) or "edge" (t0 placed per event of the second cycle by _edge_offsets).  Returns [(t0, td, ev, ctrl)]."""
+    one, period, T, N = RH_GAITS[gait]
+    ev = _cycles(one(), period, 4, sto)
+    dt = T / N
+    if which == "sweep":
+        t0s = [k * dt / per_dt for k in range(int(round(period / (dt / per_dt))))]
+    else:
+        cycle = [e[0] for e in _events_in_order(one())]
+        t0s = [period + te - off for te in cycle for off in _edge_offsets(dt, T)]
+    out = []
+    for t0 in t0s:
+        td = TimeDiscretization(T, N).discretize(ev, t0, sto=True)
+        out.append((t0, td, ev, stage_ctrl_array(td, ev)))
+    return out
+
+
+RH_SETS = (("trot", False), ("trot", True), ("crawl", False))
+
+
+def receding_horizon_coverage(schedules):
+    """Asserts that `schedules` ([(t0, td, ev, ctrl)], e.g. the sweep and edge sets of RH_SETS together) reach the grid
+    positions the kernels branch on: an impact on grid 1 (switching constraint on grid 0) with and without STO, an impact on
+    n_grid - 3, a lift on n_grid - 2, a one-grid first phase with STO, a step below 1e-5 T / N and three or more n_grid."""
+    seen, n_grids = set(), set()
+    for t0, td, ev, ctrl in schedules:
+        n = len(ctrl)
+        n_grids.add(n)
+        if ctrl[1].type == IMPACT:
+            seen.add(("impact@1", bool(ctrl[0].sto)))
+        if ctrl[0].ns > 0:
+            seen.add(("switching constraint@0", bool(ctrl[0].sto)))
+        if ctrl[n - 3].type == IMPACT:
+            seen.add("impact@n-3")
+        if ctrl[n - 2].type == LIFT:
+            seen.add("lift@n-2")
+        if ctrl[0].ngrids_in_phase == 1 and ctrl[0].sto:
+            seen.add("one-grid first phase, sto")
+        if min(c.dt for c in ctrl[:-1] if c.type != IMPACT) < 1e-5 * td.T / td.N:
+            seen.add("tiny step")
+    want = {("impact@1", False), ("impact@1", True), ("switching constraint@0", False), ("switching constraint@0", True), "impact@n-3", "lift@n-2", "one-grid first phase, sto", "tiny step"}
+    assert want <= seen, want - seen
+    assert len(n_grids) >= 3, n_grids
+    return seen, n_grids
+
+
 def dense_kkt_solve(dims, L, ctrl, kkt1, dx0):
     """Independent reference: assemble the full block KKT system of the equality-constrained LQ subproblem
     (no STO) for ONE OCP and solve it with numpy.  Returns dict of per-stage dx, du, lmd, xi."""

@@ -9,6 +9,7 @@ import ctypes
 import numpy as np
 
 import oracle_lib
+from helpers import rel_err
 from robotoc_b200 import ANYMAL
 from robotoc_b200.grid import IMPACT, TERMINAL
 
@@ -156,3 +157,160 @@ def run_device_iteration(rr, dms, lin, con, sol, dx0, stream=None):
     steps = np.stack([dms.maxPrimalStepSize(stream), dms.maxDualStepSize(stream)], axis=1)
     return dict(ric=rr.getRiccatiFactorization(stream), d=rr.getDirection(stream), steps=steps, sol=dms.getSolution(stream),
                 cc=dms.getConstraintData(stream), info=rr.info(stream))
+
+
+def compare_reference_records(S, K, ctrl, got, ref, tol, skip_sol=True, impact_cones=False):
+    """Every section the reference's code produces, stage by stage (sections it leaves untouched are not compared)."""
+    def rel(name, a, b):
+        s = float(np.max(np.abs(b)))
+        if s == 0.0:
+            assert float(np.max(np.abs(a))) == 0.0, name
+            return
+        e = float(np.max(np.abs(a - b))) / s
+        assert e < tol, f"{name}: {e:.2e}"
+    nx, nu, nv = K.nx, K.nu, K.nv
+    got, ref = dict(got), dict(ref)
+    for dct in (got, ref):  # sections nothing reads on grid points without switching-time optimisation
+        dct["kkt"] = mask_unread_sto(K, S, ctrl, kkt=np.array(dct["kkt"]))
+        dct["ex_upd"] = mask_unread_sto(K, S, ctrl, ex=np.array(dct["ex_upd"]))
+    for i, c in enumerate(ctrl):
+        rel(f"Qxx[{i}]", got["kkt"][:, i, K.k_Qxx:K.k_Qxx + nx * nx], ref["kkt"][:, i, K.k_Qxx:K.k_Qxx + nx * nx])
+        rel(f"lx[{i}]", got["kkt"][:, i, K.k_lx:K.k_lx + nx], ref["kkt"][:, i, K.k_lx:K.k_lx + nx])
+        rel(f"P[{i}]", got["ric"][:, i, K.r_P:K.r_P + nx * nx], ref["ric"][:, i, K.r_P:K.r_P + nx * nx])
+        rel(f"dx[{i}]", got["d_upd"][:, i, K.d_dx:K.d_dx + nx], ref["d_upd"][:, i, K.d_dx:K.d_dx + nx])
+        rel(f"dlmdgmm[{i}]", got["d_upd"][:, i, K.d_dlmdgmm:K.d_dlmdgmm + nx], ref["d_upd"][:, i, K.d_dlmdgmm:K.d_dlmdgmm + nx])
+        if c.type == TERMINAL:
+            continue
+        nvf = nv + c.nf
+        rel(f"kkt[{i}]", got["kkt"][:, i], ref["kkt"][:, i])
+        for f, n in (("e_Z", S.nvf * S.nvf), ("e_R", S.nvf * nx), ("e_r", nvf), ("e_Qafqv", S.nvf * nx), ("e_laf", nvf), ("e_Fqqpi", 36)):
+            o = getattr(S, f)
+            rel(f"{f}[{i}]", got["ex_upd"][:, i, o:o + n], ref["ex_upd"][:, i, o:o + n])
+        rel(f"daf[{i}]", got["xd_exp"][:, i, S.x_daf:S.x_daf + nvf], ref["xd_exp"][:, i, S.x_daf:S.x_daf + nvf])
+        rel(f"dbetamu[{i}]", got["xd_upd"][:, i, S.x_dbetamu:S.x_dbetamu + nvf], ref["xd_upd"][:, i, S.x_dbetamu:S.x_dbetamu + nvf])
+        if c.type == IMPACT:
+            if impact_cones:  # the ImpactFrictionCone rows (the box rows do not exist on an impact stage)
+                for key, fields in (("cc_cond", ("c_cmpl", "c_cond")), ("cc_exp", ("c_dslack", "c_ddual")), ("cc_upd", ("c_slack", "c_dual"))):
+                    for f in fields:
+                        o = getattr(S, f)
+                        rel(f"impact {f}[{i}]", got[key][:, i, o + S.nbox:o + S.nc], ref[key][:, i, o + S.nbox:o + S.nc])
+            continue
+        for f, n in (("e_Qafu", S.nvf * nv), ("e_Qxup", nx * S.np), ("e_Quup", S.np * nu), ("e_lup", S.np), ("e_haf", nvf)):
+            o = getattr(S, f)
+            rel(f"{f}[{i}]", got["ex_upd"][:, i, o:o + n], ref["ex_upd"][:, i, o:o + n])
+        rel(f"dnup[{i}]", got["xd_upd"][:, i, S.x_dnup:S.x_dnup + S.np], ref["xd_upd"][:, i, S.x_dnup:S.x_dnup + S.np])
+        rel(f"K[{i}]", got["ric"][:, i, K.r_K:K.r_K + nx * nu], ref["ric"][:, i, K.r_K:K.r_K + nx * nu])
+        rel(f"du[{i}]", got["d_upd"][:, i, K.d_du:K.d_du + nu], ref["d_upd"][:, i, K.d_du:K.d_du + nu])
+        for key, fields in (("cc_cond", ("c_cmpl", "c_cond")), ("cc_exp", ("c_dslack", "c_ddual")), ("cc_upd", ("c_slack", "c_dual"))):
+            for f in fields:
+                o = getattr(S, f)
+                rel(f"{f}[{i}]", got[key][:, i, o:o + S.nc], ref[key][:, i, o:o + S.nc])
+    rel("steps", got["steps"], ref["steps"])
+
+
+def cuda_iteration_records(rr, dms, S, lin, con, sol, dx0):
+    """One iteration through the C ABI, every record the reference iteration stores."""
+    dms.condense(lin, con)
+    got = dict(kkt=dms.getKKT(), cc_cond=dms.getConstraintData())
+    rr.backwardRiccatiRecursion()
+    rr.forwardRiccatiRecursion(dx0)
+    assert int(rr.info().max()) == 0
+    got["ric"] = rr.getRiccatiFactorization()
+    dms.computeStepSizes()
+    got["steps"] = np.stack([dms.maxPrimalStepSize(), dms.maxDualStepSize()], axis=1)
+    got["cc_exp"], got["xd_exp"] = dms.getConstraintData(), dms.getExpandedDirection()
+    dms.integrateSolution(sol)
+    got["d_upd"], got["xd_upd"], got["cc_upd"], got["ex_upd"] = (rr.getDirection(), dms.getExpandedDirection(), dms.getConstraintData(),
+                                                                 reference_view_of_expansion(S, dms.getExpansionData()))
+    return got
+
+
+def riccati_blocks(L, d, c):
+    nx, nu, ns = d.nx, d.nu, c.ns
+    b = {"P": (L.r_P, nx * nx), "s": (L.r_s, nx)}
+    if c.type != IMPACT and c.type != 3:
+        b.update({"K": (L.r_K, nx * nu), "k": (L.r_k, nu)})
+        if ns > 0:
+            b.update({"M": (L.r_M, ns * nx), "m": (L.r_m, ns)})
+    if c.sto:
+        b.update({"Psi": (L.r_Psi, nx), "Phi": (L.r_Phi, nx), "sc": (L.r_sc, 5)})
+        if c.type != IMPACT:
+            b.update({"T": (L.r_T, nu), "W": (L.r_W, nu), "psix": (L.r_psix, nx), "psiu": (L.r_psiu, nu),
+                      "phix": (L.r_phix, nx), "phiu": (L.r_phiu, nu)})
+            if ns > 0:
+                b.update({"mt": (L.r_mt, ns), "mtn": (L.r_mtn, ns)})
+    b.update({"dtsdx": (L.r_dtsdx, nx), "stosc": (L.r_stosc, 2)})
+    return b
+
+
+def compare_riccati(dims, L, ctrl, got_ric, ref_ric, got_d, ref_d, got_f=None, ref_kkt=None, tol=1e-8):
+    """Every block of the Riccati factorization, the direction and (if given) the factorized KKT records against the oracle's,
+    stage by stage, relative to each block's scale.  Returns the worst error."""
+    worst = 0.0
+    for i, c in enumerate(ctrl):
+        for name, (off, n) in riccati_blocks(L, dims, c).items():
+            a, b = got_ric[:, i, off:off + n], ref_ric[:, i, off:off + n]
+            if np.max(np.abs(b)) == 0.0:
+                assert np.max(np.abs(a)) == 0.0, f"stage {i} block {name}: expected zeros"
+                continue
+            if name == "W" and c.ns == dims.nu:
+                # ns == nu: the projected inverse Ginv - SDG^T DG is analytically zero, so W = -Ginv phi_u is pure
+                # cancellation noise (~1e-14); compare on the scale of its sibling T instead of its own.
+                scale = np.max(np.abs(ref_ric[:, i, L.r_T:L.r_T + dims.nu]))
+                assert np.max(np.abs(a - b)) < 1e-9 * scale, f"riccati stage {i} block W (ns==nu)"
+                continue
+            e = rel_err(a, b)
+            worst = max(worst, e)
+            assert e < tol, f"riccati stage {i} block {name}: rel err {e:.3e}"
+        dblocks = {"dx": (L.d_dx, dims.nx), "dlmdgmm": (L.d_dlmdgmm, dims.nx), "dts": (L.d_dts, 2)}
+        if c.type not in (IMPACT, 3):
+            dblocks["du"] = (L.d_du, dims.nu)
+            if c.ns > 0:
+                dblocks["dxi"] = (L.d_dxi, c.ns)
+        for name, (off, n) in dblocks.items():
+            a, b = got_d[:, i, off:off + n], ref_d[:, i, off:off + n]
+            if np.max(np.abs(b)) == 0.0:
+                assert np.max(np.abs(a)) < 1e-300, f"stage {i} dir {name}: expected zeros"
+                continue
+            e = rel_err(a, b)
+            worst = max(worst, e)
+            assert e < tol, f"direction stage {i} block {name}: rel err {e:.3e}"
+        if got_f is not None and c.type != 3:
+            fb = {"F": (L.f_F, L.k_Qxx, dims.nx ** 2)}
+            if c.type != IMPACT:
+                fb.update({"H": (L.f_H, L.k_Qxu, dims.nx * dims.nu), "G": (L.f_G, L.k_Quu, dims.nu ** 2),
+                           "lu": (L.f_lu, L.k_lu, dims.nu)})
+            for name, (fo, ko, n) in fb.items():
+                e = rel_err(got_f[:, i, fo:fo + n], ref_kkt[:, i, ko:ko + n])
+                worst = max(worst, e)
+                assert e < tol, f"factorized KKT stage {i} block {name}: rel err {e:.3e}"
+    return worst
+
+
+def oracle_perf_index(lib, sd, table, ctrl, lin, con):
+    """The oracle's PerformanceIndex of evalKKT per OCP: the eight values rbt_eval_kkt returns."""
+    lib.orc_perf_index_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 3
+    perf = np.zeros((lin.shape[0], 8))
+    csd = sd.c()
+    lib.orc_perf_index_batch(ctypes.byref(csd), ctypes.byref(table), ctrl, len(ctrl), lin.shape[0], oracle_lib.ptr(lin),
+                             oracle_lib.ptr(con), oracle_lib.ptr(perf))
+    return perf
+
+
+TRIAL_STRIDE = 80  # doubles per grid point of a line-search trial record: q | v | a (dv) | u | f
+
+
+def oracle_trials(lib, sd, table, ctrl, sol, ref, n_trials, rate=0.75):
+    """The oracle's line-search trials from the iterate `sol` along the direction of `ref` (oracle_iteration): step sizes,
+    log barrier and trial records [n_trials, batch, n_grid, TRIAL_STRIDE]."""
+    vp, ci, cd = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
+    lib.orc_trial_batch.argtypes = [vp, vp, vp, ci, ci, ci, cd] + [vp] * 8
+    batch, n_grid = sol.shape[0], sol.shape[1]
+    alphas, barrier = np.zeros((n_trials, batch)), np.zeros((n_trials, batch))
+    trial = np.zeros((n_trials, batch, n_grid, TRIAL_STRIDE))
+    csd = sd.c()
+    P = oracle_lib.ptr
+    lib.orc_trial_batch(ctypes.byref(csd), ctypes.byref(table), ctrl, n_grid, batch, n_trials, rate, P(sol), P(ref["d"]), P(ref["xd_exp"]),
+                        P(ref["cc_exp"]), P(ref["steps"]), P(alphas), P(trial), P(barrier))
+    return alphas, barrier, trial
+

@@ -135,3 +135,34 @@ def reference_iteration(sd, S, K, table, ctrl, lin, con, dx0):
             d_upd[b, i], xd_upd[b, i], cc_upd[b, i], ex_upd[b, i] = o["d"], o["xd"], o["con"], o["ex"]
     return dict(kkt=kkt, cc_cond=cc_cond, ric=ric, d=d, cc_exp=cc_exp, xd_exp=xd_exp, steps=steps, d_upd=d_upd, xd_upd=xd_upd,
                 cc_upd=cc_upd, ex_upd=ex_upd, perf_stage=perf_stage)
+
+
+LIB_DISCRETIZE = os.path.join(ORACLE_DIR, "_ref", "libref_discretize.so")
+_lib_td = None
+
+
+def discretize(T, N, ev, t0, phase_based=True):
+    """robotoc::TimeDiscretization::discretize(t0) (+ correctTimeSteps(t0) if `phase_based`) of the reference, on the
+    ContactSequence that `ev` (schedule_fixture.ContactEvents) describes (oracle/ref_wrap/ref_discretize_wrap.cpp).  Returns
+    one dict of GridInfo fields per grid point."""
+    global _lib_td
+    if _lib_td is None:
+        build()
+        L = ctypes.CDLL(LIB_DISCRETIZE)
+        c_int, c_dbl, c_vp = ctypes.c_int, ctypes.c_double, ctypes.c_void_p
+        L.ref_discretize.argtypes = [c_dbl, c_int, c_int, c_vp, c_vp, c_vp, c_dbl, c_int, c_int, c_vp, c_vp]
+        _lib_td = L
+    events = sorted([(t, s) for t, s in zip(ev.impact_times, ev.sto_impact)] + [(t, s) for t, s in zip(ev.lift_times, ev.sto_lift)])
+    masks = np.array(ev.phase_mask, dtype=np.int32)
+    times = np.array([t for t, _ in events], dtype=np.float64)
+    sto = np.array([int(s) for _, s in events], dtype=np.int32)
+    n_max = N + 1 + 3 * len(events) + 1
+    ints, dbls = np.zeros((n_max, 10), dtype=np.int32), np.zeros((n_max, 4))
+    n = _lib_td.ref_discretize(T, N, len(events), masks.ctypes.data, times.ctypes.data, sto.ctypes.data, t0, int(phase_based),
+                               n_max, ints.ctypes.data, dbls.ctypes.data)
+    assert n > 0, f"ref_discretize failed ({n})"
+    names_i = ("type", "phase", "stage", "impact_index", "lift_index", "stage_in_phase", "num_grids_in_phase", "sto", "sto_next",
+               "switching_constraint")
+    names_d = ("t0", "t", "dt", "dt_next")
+    return [dict(**{k: int(v) for k, v in zip(names_i, ints[i])}, **{k: float(v) for k, v in zip(names_d, dbls[i])})
+            for i in range(n)]

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import oracle_lib
+from iteration_check import oracle_perf_index as _oracle_perf
 from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedule, small_event_schedule, trot_schedule
 from robotoc_b200 import ANYMAL, StageDims, StageLayout, anymal_constraint_table
 from robotoc_b200.grid import IMPACT, TERMINAL
@@ -29,14 +30,6 @@ def _setup(sched, batch, seed, getter=None, impact_cones=False):
     lib.orc_set_slack_dual_positive_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     lib.orc_initial_state_direction.argtypes = [ctypes.c_void_p] + [ctypes.c_void_p] * 5
     return lib, table, sd, S, ctrl, lin, con, sol, dx0
-
-
-def _oracle_perf(lib, sd, table, ctrl, lin, con):
-    perf = np.zeros((lin.shape[0], 8))
-    csd = sd.c()
-    lib.orc_perf_index_batch(ctypes.byref(csd), ctypes.byref(table), ctrl, len(ctrl), lin.shape[0], oracle_lib.ptr(lin),
-                             oracle_lib.ptr(con), oracle_lib.ptr(perf))
-    return perf
 
 
 def _numpy_perf(S, table, ctrl, lin, con):

@@ -17,8 +17,8 @@ from golden_sample import load, restore  # noqa: E402
 import make_golden_ref_live as mgl  # noqa: E402
 
 import oracle_lib  # noqa: E402
-from iteration_check import mask_unread_sto, oracle_iteration, reference_view_of_expansion  # noqa: E402
-from robotoc_b200.grid import IMPACT, TERMINAL  # noqa: E402
+from iteration_check import compare_reference_records as _cmp_records, cuda_iteration_records as _cuda_iteration  # noqa: E402
+from iteration_check import oracle_iteration  # noqa: E402
 
 G = load(mg.PATH)
 
@@ -28,55 +28,6 @@ def _golden(got, impact_cones):
     pre = "ic_" if impact_cones else ""
     return {k: restore(G, pre + k, got[k]) for k in mg.KEYS if k in got}
 TOL = 1e-10
-
-
-def _cmp_records(S, K, ctrl, got, ref, tol, skip_sol=True, impact_cones=False):
-    """Every section the reference's code produces, stage by stage (sections it leaves untouched are not compared)."""
-    def rel(name, a, b):
-        s = float(np.max(np.abs(b)))
-        if s == 0.0:
-            assert float(np.max(np.abs(a))) == 0.0, name
-            return
-        e = float(np.max(np.abs(a - b))) / s
-        assert e < tol, f"{name}: {e:.2e}"
-    nx, nu, nv = K.nx, K.nu, K.nv
-    got, ref = dict(got), dict(ref)
-    for dct in (got, ref):  # sections nothing reads on grid points without switching-time optimisation
-        dct["kkt"] = mask_unread_sto(K, S, ctrl, kkt=np.array(dct["kkt"]))
-        dct["ex_upd"] = mask_unread_sto(K, S, ctrl, ex=np.array(dct["ex_upd"]))
-    for i, c in enumerate(ctrl):
-        rel(f"Qxx[{i}]", got["kkt"][:, i, K.k_Qxx:K.k_Qxx + nx * nx], ref["kkt"][:, i, K.k_Qxx:K.k_Qxx + nx * nx])
-        rel(f"lx[{i}]", got["kkt"][:, i, K.k_lx:K.k_lx + nx], ref["kkt"][:, i, K.k_lx:K.k_lx + nx])
-        rel(f"P[{i}]", got["ric"][:, i, K.r_P:K.r_P + nx * nx], ref["ric"][:, i, K.r_P:K.r_P + nx * nx])
-        rel(f"dx[{i}]", got["d_upd"][:, i, K.d_dx:K.d_dx + nx], ref["d_upd"][:, i, K.d_dx:K.d_dx + nx])
-        rel(f"dlmdgmm[{i}]", got["d_upd"][:, i, K.d_dlmdgmm:K.d_dlmdgmm + nx], ref["d_upd"][:, i, K.d_dlmdgmm:K.d_dlmdgmm + nx])
-        if c.type == TERMINAL:
-            continue
-        nvf = nv + c.nf
-        rel(f"kkt[{i}]", got["kkt"][:, i], ref["kkt"][:, i])
-        for f, n in (("e_Z", S.nvf * S.nvf), ("e_R", S.nvf * nx), ("e_r", nvf), ("e_Qafqv", S.nvf * nx), ("e_laf", nvf), ("e_Fqqpi", 36)):
-            o = getattr(S, f)
-            rel(f"{f}[{i}]", got["ex_upd"][:, i, o:o + n], ref["ex_upd"][:, i, o:o + n])
-        rel(f"daf[{i}]", got["xd_exp"][:, i, S.x_daf:S.x_daf + nvf], ref["xd_exp"][:, i, S.x_daf:S.x_daf + nvf])
-        rel(f"dbetamu[{i}]", got["xd_upd"][:, i, S.x_dbetamu:S.x_dbetamu + nvf], ref["xd_upd"][:, i, S.x_dbetamu:S.x_dbetamu + nvf])
-        if c.type == IMPACT:
-            if impact_cones:  # the ImpactFrictionCone rows (the box rows do not exist on an impact stage)
-                for key, fields in (("cc_cond", ("c_cmpl", "c_cond")), ("cc_exp", ("c_dslack", "c_ddual")), ("cc_upd", ("c_slack", "c_dual"))):
-                    for f in fields:
-                        o = getattr(S, f)
-                        rel(f"impact {f}[{i}]", got[key][:, i, o + S.nbox:o + S.nc], ref[key][:, i, o + S.nbox:o + S.nc])
-            continue
-        for f, n in (("e_Qafu", S.nvf * nv), ("e_Qxup", nx * S.np), ("e_Quup", S.np * nu), ("e_lup", S.np), ("e_haf", nvf)):
-            o = getattr(S, f)
-            rel(f"{f}[{i}]", got["ex_upd"][:, i, o:o + n], ref["ex_upd"][:, i, o:o + n])
-        rel(f"dnup[{i}]", got["xd_upd"][:, i, S.x_dnup:S.x_dnup + S.np], ref["xd_upd"][:, i, S.x_dnup:S.x_dnup + S.np])
-        rel(f"K[{i}]", got["ric"][:, i, K.r_K:K.r_K + nx * nu], ref["ric"][:, i, K.r_K:K.r_K + nx * nu])
-        rel(f"du[{i}]", got["d_upd"][:, i, K.d_du:K.d_du + nu], ref["d_upd"][:, i, K.d_du:K.d_du + nu])
-        for key, fields in (("cc_cond", ("c_cmpl", "c_cond")), ("cc_exp", ("c_dslack", "c_ddual")), ("cc_upd", ("c_slack", "c_dual"))):
-            for f in fields:
-                o = getattr(S, f)
-                rel(f"{f}[{i}]", got[key][:, i, o:o + S.nc], ref[key][:, i, o:o + S.nc])
-    rel("steps", got["steps"], ref["steps"])
 
 
 @pytest.mark.parametrize("impact_cones", [False, True])
@@ -132,6 +83,27 @@ def test_oracle_equals_live_reference_stage_layer(which, seed):
     _cmp_records(S, K, ctrl, got, ref, TOL, impact_cones=icone)
 
 
+def test_oracle_equals_live_reference_on_horizon_edges():
+    """The receding-horizon edge schedules (t0 != 0, events on grid 1 and beside it, at the last admissible grid points, steps
+    far below T / N; with and without impact cones): the oracle == the reference's code (golden_ref_horizon.npz)."""
+    lib = oracle_lib.load()
+    GH = load(mgl.HORIZON_PATH)
+    for case in mgl.horizon_cases():
+        table, sd, S, K, ctrl, lin, con, sol, dx0, icone = mgl.horizon_case(case, lib.orc_stage_layout_get, lib.orc_layout_get)
+        got = oracle_iteration(sd, S, K, table, ctrl, lin, con, sol, dx0)
+        ref = {k: restore(GH, f"h_{case[0]}_{k}", got[k]) for k in mgl.STAGE_KEYS}
+        try:
+            _cmp_records(S, K, ctrl, got, ref, TOL, impact_cones=icone)
+        except AssertionError as e:
+            raise AssertionError(f"{case[0]} t0={case[3]!r} (n_grid {len(ctrl)}): {e}") from None
+
+
+def test_horizon_edge_cases_cover_the_edges():
+    """The edge cases stored in golden_ref_horizon.npz reach the grid positions the kernels branch on."""
+    from helpers import receding_horizon_coverage
+    receding_horizon_coverage([(c[3], c[4], None, c[5]) for c in mgl.horizon_cases()])
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("impact_cones", [False, True])
 def test_cuda_reproduces_the_reference_iteration_golden(impact_cones):
@@ -148,23 +120,6 @@ def test_cuda_reproduces_the_reference_iteration_golden(impact_cones):
     got = _cuda_iteration(rr, dms, S, lin, con, sol, dx0)
     _cmp_records(S, K, ctrl, got, _golden(got, impact_cones), 1e-8, impact_cones=impact_cones)
     rr.close()
-
-
-def _cuda_iteration(rr, dms, S, lin, con, sol, dx0):
-    """One iteration through the C ABI, every record the reference iteration stores."""
-    dms.condense(lin, con)
-    got = dict(kkt=dms.getKKT(), cc_cond=dms.getConstraintData())
-    rr.backwardRiccatiRecursion()
-    rr.forwardRiccatiRecursion(dx0)
-    assert int(rr.info().max()) == 0
-    got["ric"] = rr.getRiccatiFactorization()
-    dms.computeStepSizes()
-    got["steps"] = np.stack([dms.maxPrimalStepSize(), dms.maxDualStepSize()], axis=1)
-    got["cc_exp"], got["xd_exp"] = dms.getConstraintData(), dms.getExpandedDirection()
-    dms.integrateSolution(sol)
-    got["d_upd"], got["xd_upd"], got["cc_upd"], got["ex_upd"] = (rr.getDirection(), dms.getExpandedDirection(), dms.getConstraintData(),
-                                                                 reference_view_of_expansion(S, dms.getExpansionData()))
-    return got
 
 
 @pytest.mark.gpu

@@ -8,70 +8,11 @@ from helpers import contact_mask_walk_schedule, crawl_schedule, jump_sto_schedul
 from robotoc_b200 import ANYMAL, Layout, RiccatiRecursion, ULayout, UnconstrRiccatiRecursion
 from robotoc_b200 import _lib
 from robotoc_b200.grid import IMPACT, INTERMEDIATE
+from iteration_check import compare_riccati as _compare
 from synth import make_kkt, make_unconstr_kkt
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-8
-
-
-def _blocks_ric(L, d, c):
-    nx, nu, ns = d.nx, d.nu, c.ns
-    b = {"P": (L.r_P, nx * nx), "s": (L.r_s, nx)}
-    if c.type != IMPACT and c.type != 3:
-        b.update({"K": (L.r_K, nx * nu), "k": (L.r_k, nu)})
-        if ns > 0:
-            b.update({"M": (L.r_M, ns * nx), "m": (L.r_m, ns)})
-    if c.sto:
-        b.update({"Psi": (L.r_Psi, nx), "Phi": (L.r_Phi, nx), "sc": (L.r_sc, 5)})
-        if c.type != IMPACT:
-            b.update({"T": (L.r_T, nu), "W": (L.r_W, nu), "psix": (L.r_psix, nx), "psiu": (L.r_psiu, nu),
-                      "phix": (L.r_phix, nx), "phiu": (L.r_phiu, nu)})
-            if ns > 0:
-                b.update({"mt": (L.r_mt, ns), "mtn": (L.r_mtn, ns)})
-    b.update({"dtsdx": (L.r_dtsdx, nx), "stosc": (L.r_stosc, 2)})
-    return b
-
-
-def _compare(dims, L, ctrl, got_ric, ref_ric, got_d, ref_d, got_f=None, ref_kkt=None, tol=TOL):
-    worst = 0.0
-    for i, c in enumerate(ctrl):
-        for name, (off, n) in _blocks_ric(L, dims, c).items():
-            a, b = got_ric[:, i, off:off + n], ref_ric[:, i, off:off + n]
-            if np.max(np.abs(b)) == 0.0:
-                assert np.max(np.abs(a)) == 0.0, f"stage {i} block {name}: expected zeros"
-                continue
-            if name == "W" and c.ns == dims.nu:
-                # ns == nu: the projected inverse Ginv - SDG^T DG is analytically zero, so W = -Ginv phi_u is pure
-                # cancellation noise (~1e-14); compare on the scale of its sibling T instead of its own.
-                scale = np.max(np.abs(ref_ric[:, i, L.r_T:L.r_T + dims.nu]))
-                assert np.max(np.abs(a - b)) < 1e-9 * scale, f"riccati stage {i} block W (ns==nu)"
-                continue
-            e = rel_err(a, b)
-            worst = max(worst, e)
-            assert e < tol, f"riccati stage {i} block {name}: rel err {e:.3e}"
-        dblocks = {"dx": (L.d_dx, dims.nx), "dlmdgmm": (L.d_dlmdgmm, dims.nx), "dts": (L.d_dts, 2)}
-        if c.type not in (IMPACT, 3):
-            dblocks["du"] = (L.d_du, dims.nu)
-            if c.ns > 0:
-                dblocks["dxi"] = (L.d_dxi, c.ns)
-        for name, (off, n) in dblocks.items():
-            a, b = got_d[:, i, off:off + n], ref_d[:, i, off:off + n]
-            if np.max(np.abs(b)) == 0.0:
-                assert np.max(np.abs(a)) < 1e-300, f"stage {i} dir {name}: expected zeros"
-                continue
-            e = rel_err(a, b)
-            worst = max(worst, e)
-            assert e < tol, f"direction stage {i} block {name}: rel err {e:.3e}"
-        if got_f is not None and c.type != 3:
-            fb = {"F": (L.f_F, L.k_Qxx, dims.nx ** 2)}
-            if c.type != IMPACT:
-                fb.update({"H": (L.f_H, L.k_Qxu, dims.nx * dims.nu), "G": (L.f_G, L.k_Quu, dims.nu ** 2),
-                           "lu": (L.f_lu, L.k_lu, dims.nu)})
-            for name, (fo, ko, n) in fb.items():
-                e = rel_err(got_f[:, i, fo:fo + n], ref_kkt[:, i, ko:ko + n])
-                worst = max(worst, e)
-                assert e < tol, f"factorized KKT stage {i} block {name}: rel err {e:.3e}"
-    return worst
 
 
 def _run_case(ctrl, batch, seed, max_dts0=0.1):

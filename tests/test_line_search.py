@@ -13,12 +13,12 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "gol
 import make_golden_ref_live as mgl  # noqa: E402
 import oracle_lib  # noqa: E402
 from helpers import contact_mask_walk_schedule, crawl_schedule, small_event_schedule, trot_schedule
-from iteration_check import oracle_iteration
+from iteration_check import TRIAL_STRIDE, oracle_iteration, oracle_trials
 from robotoc_b200 import ANYMAL, Layout, StageDims, StageLayout, anymal_constraint_table
 from robotoc_b200.grid import IMPACT, TERMINAL
 from synth import make_stage_inputs
 
-T_Q, T_V, T_A, T_U, T_F, T_STRIDE = 0, 20, 38, 56, 68, 80
+T_Q, T_V, T_A, T_U, T_F, T_STRIDE = 0, 20, 38, 56, 68, TRIAL_STRIDE
 CAP = 16
 
 
@@ -69,14 +69,7 @@ def _problem(sched, batch, seed, getter=True, impact_cones=False):
 
 
 def _oracle_trials(lib, sd, table, ctrl, S, K, sol, ref, n_trials, rate=0.75):
-    batch, n_grid = sol.shape[0], sol.shape[1]
-    alphas, barrier = np.zeros((n_trials, batch)), np.zeros((n_trials, batch))
-    trial = np.zeros((n_trials, batch, n_grid, T_STRIDE))
-    csd = sd.c()
-    P = oracle_lib.ptr
-    lib.orc_trial_batch(ctypes.byref(csd), ctypes.byref(table), ctrl, n_grid, batch, n_trials, rate, P(sol), P(ref["d"]), P(ref["xd_exp"]),
-                        P(ref["cc_exp"]), P(ref["steps"]), P(alphas), P(trial), P(barrier))
-    return alphas, barrier, trial
+    return oracle_trials(lib, sd, table, ctrl, sol, ref, n_trials, rate)
 
 
 @pytest.mark.parametrize("impact_cones", [False, True])
