@@ -348,7 +348,11 @@ int rbt_unconstr_solve_host(rbt_uhandle* h, const double* kkt_host, const double
 int rbt_unconstr_stage_layout_get(int nv, int n_box, const char* field);
 int rbt_unconstr_stage_setup(rbt_uhandle* h, const rbt_constraint_table* table);
 /* Constraints::condenseSlackAndDual + UnconstrDynamics::condenseUnconstrDynamics (src/dynamics/unconstr_dynamics.cpp:67-87)
- * on every stage; terminal stage: Qxx, lx.  Reads RBT_BUF_LIN, RBT_BUF_CON; writes RBT_BUF_KKT, RBT_BUF_EXP, RBT_BUF_CON. */
+ * on every stage; terminal stage: Qxx, lx.  Reads RBT_BUF_LIN, RBT_BUF_CON; writes RBT_BUF_KKT, RBT_BUF_EXP, RBT_BUF_CON.
+ * As ConstraintsData::setTimeStage does for GridInfo::stage = i (constraints_data.cpp:20-45), a table row acts on stage i iff
+ * i >= 2 for RBT_VAR_Q, i >= 1 for RBT_VAR_V, always for RBT_VAR_A / RBT_VAR_U; the PDIPM record of a row that does not act is
+ * left untouched by this call, rbt_unconstr_expand_and_step_sizes (which also leaves it out of the step sizes) and
+ * rbt_unconstr_update. */
 int rbt_unconstr_condense(rbt_uhandle* h, void* stream);
 /* UnconstrDirectMultipleShooting::computeStepSizes + maxPrimalStepSize / maxDualStepSize (:128-156): expandPrimal, expandDual
  * (unconstr_dynamics.cpp:90-104), slack/dual directions, fraction-to-boundary, min over the horizon -> RBT_BUF_STEPS. */

@@ -81,6 +81,22 @@ class Robot {
 #define RBT_SHIM_UNREACHABLE(NAME) { std::fprintf(stderr, "oracle/shim Robot::" NAME " called: Pinocchio is not available\n"); std::abort(); }
   template <typename... A> void RNEA(const A&...) RBT_SHIM_UNREACHABLE("RNEA")
   template <typename... A> void RNEADerivatives(const A&...) RBT_SHIM_UNREACHABLE("RNEADerivatives")
+  /// Test hook for a fixed-base robot: UnconstrDynamics keeps ID_ and dID_d* private and fills them only through
+  /// RNEA / RNEADerivatives (unconstr_dynamics.cpp:46-60).  These overloads (exact matches for the VectorXd / MatrixXd members,
+  /// so they win over the aborting templates above) return the injected values, which are INPUTS of the hot path (sections
+  /// l_ID, l_dIDd* of the unconstrained linearization record).
+  void injectRNEA(const Eigen::VectorXd& ID, const Eigen::MatrixXd& dq, const Eigen::MatrixXd& dv, const Eigen::MatrixXd& da) {
+    inj_ID_ = ID; inj_dq_ = dq; inj_dv_ = dv; inj_da_ = da; has_inj_rnea_ = true;
+  }
+  void RNEA(const Eigen::VectorXd&, const Eigen::VectorXd&, const Eigen::VectorXd&, Eigen::VectorXd& tau) {
+    if (!has_inj_rnea_) RBT_SHIM_UNREACHABLE("RNEA without injected values")
+    tau = inj_ID_;
+  }
+  void RNEADerivatives(const Eigen::VectorXd&, const Eigen::VectorXd&, const Eigen::VectorXd&, Eigen::MatrixXd& dq,
+                       Eigen::MatrixXd& dv, Eigen::MatrixXd& da) {
+    if (!has_inj_rnea_) RBT_SHIM_UNREACHABLE("RNEADerivatives without injected values")
+    dq = inj_dq_; dv = inj_dv_; da = inj_da_;
+  }
   template <typename... A> void RNEAImpact(const A&...) RBT_SHIM_UNREACHABLE("RNEAImpact")
   template <typename... A> void RNEAImpactDerivatives(const A&...) RBT_SHIM_UNREACHABLE("RNEAImpactDerivatives")
   template <typename... A> void updateKinematics(const A&...) RBT_SHIM_UNREACHABLE("updateKinematics")
@@ -137,6 +153,9 @@ class Robot {
   Eigen::VectorXd limit_effort_, limit_velocity_, limit_qmin_, limit_qmax_;
   Eigen::MatrixXd injected_;
   bool has_injected_ = false;
+  Eigen::VectorXd inj_ID_;
+  Eigen::MatrixXd inj_dq_, inj_dv_, inj_da_;
+  bool has_inj_rnea_ = false;
 };
 
 }  // namespace robotoc

@@ -4,11 +4,17 @@
  * TEST INFRASTRUCTURE ONLY: used by tests/, __graft_entry__.smoke() and bench.py's CPU legs as the checker.  The product
  * (librobotoc_b200.so) never links or calls it.
  *
- * Parity pinning: the reference (Eigen + Pinocchio + cmake) cannot be built in this image, so this file is pinned by
- * tests/test_oracle_unconstr_stage.py through reference-independent identities: the condensed (q,v,a) model equals the
- * (q,v,a,u) model with u = ID + dID*[dq;dv;da] substituted (value, gradient, Hessian), the PDIPM rows equal J^T W J /
- * J^T cond, and the expansion reproduces the Newton step of the full stage KKT system.  No golden vector from a reference
- * BINARY exists: "parity unpinned" in the sense of the task statement.
+ * Parity pinning: tests/golden/golden_ref_ustage.npz holds what the reference's own stage-layer code computes on these records
+ * (oracle/ref_wrap/ref_ustage_wrap.cpp, built by oracle/Makefile.ref), and tests/test_golden_ref_ustage.py compares this file
+ * with it block by block.  tests/test_oracle_unconstr_stage.py adds reference-independent identities: the condensed (q,v,a)
+ * model equals the (q,v,a,u) model with u = ID + dID*[dq;dv;da] substituted (value, gradient, Hessian), the PDIPM rows equal
+ * J^T W J / J^T cond, and the expansion reproduces the Newton step of the full stage KKT system.
+ *
+ * Which rows act on grid point i (GridInfo::stage = i, unconstr_ocp_solver.cpp:41-50): ConstraintsData::setTimeStage
+ * (constraints_data.cpp:20-45) turns position-level components off on stages 0 and 1 and velocity-level components off on
+ * stage 0, and every Constraints member skips a level that is not valid.  So a row of level l (2: q, 1: v, 0: a and u) acts
+ * iff i >= l; a row that does not act adds nothing to the KKT and expansion records, takes no part in the step sizes, and
+ * its PDIPM record (slack, dual, res, cmpl, cond, dslack, ddual) is left as it came in.
  *
  * Records: include/rbt_ustage_layout.h (stage layer), rbt_ulayout in include/rbt_layout.h (KKT / direction).
  */
@@ -20,6 +26,11 @@
 #include "../include/rbt_ustage_layout.h"
 
 #define IDX(i, j, ld) ((size_t)(i) + (size_t)(j) * (size_t)(ld))
+
+/* ConstraintsData::setTimeStage: does box row b act on grid point `stage`? */
+static int row_acts(const rbt_box_row* b, int stage) {
+  return stage >= (b->var == RBT_VAR_Q ? 2 : b->var == RBT_VAR_V ? 1 : 0);
+}
 
 /* C(m x n) (+)= A^T(m x k) * diag(w) * B(k x n) ; all column-major with leading dimension ld = k or given */
 static void atdb(int m, int n, int k, const double* A, const double* w, const double* B, double beta, double* C, int ldc) {
@@ -36,10 +47,10 @@ static void atdb(int m, int n, int k, const double* A, const double* w, const do
  *   pdipm::computeComplementarySlackness / condenseSlackAndDual          pdipm.hxx:27-100, joint_*_limit.cpp:68-83
  *   UnconstrDynamics::condenseUnconstrDynamics                           src/dynamics/unconstr_dynamics.cpp:67-87
  * UnconstrTerminalStage::evalKKT has no constraints and no dynamics      src/unconstr/unconstr_terminal_stage.cpp:69-94
- * terminal != 0: kkt gets Qxx, lx only.
+ * terminal != 0: kkt gets Qxx, lx only.  stage: GridInfo::stage of the grid point (row_acts).
  */
-void orc_ustage_condense(int nv, const rbt_constraint_table* tab, int terminal, const double* lin, double* con,
-                         double* kkt, double* ex) {
+void orc_ustage_condense_at(int nv, const rbt_constraint_table* tab, int stage, int terminal, const double* lin, double* con,
+                            double* kkt, double* ex) {
   rbt_ustage_layout S;
   rbt_ulayout K;
   rbt_make_ustage_layout(nv, tab->n_box, &S);
@@ -70,6 +81,7 @@ void orc_ustage_condense(int nv, const rbt_constraint_table* tab, int terminal, 
   double* cond = con + S.c_cond;
   for (int r = 0; r < tab->n_box; ++r) {
     const rbt_box_row* b = &tab->box[r];
+    if (!row_acts(b, stage)) continue;
     cmpl[r] = slack[r] * dual[r] - tab->barrier;                        /* pdipm.hxx:27-31 */
     cond[r] = (dual[r] * res[r] - cmpl[r]) / slack[r];                  /* pdipm.hxx:66-70 */
     const double w = dual[r] / slack[r];
@@ -113,11 +125,12 @@ void orc_ustage_condense(int nv, const rbt_constraint_table* tab, int terminal, 
   free(w);
 }
 
-/* pdipm::fractionToBoundary  pdipm.hxx:121-142 */
-static double fraction_to_boundary(int n, double rate, const double* v, const double* dv) {
+/* pdipm::fractionToBoundary  pdipm.hxx:121-142, over the rows that act on grid point `stage` */
+static double fraction_to_boundary(const rbt_constraint_table* tab, int stage, const double* v, const double* dv) {
   double m = 1.0;
-  for (int i = 0; i < n; ++i) {
-    const double f = -rate * (v[i] / dv[i]);
+  for (int i = 0; i < tab->n_box; ++i) {
+    if (!row_acts(&tab->box[i], stage)) continue;
+    const double f = -tab->fraction_to_boundary * (v[i] / dv[i]);
     if (f > 0 && f < 1 && f < m) m = f;
   }
   return m;
@@ -130,8 +143,8 @@ static double fraction_to_boundary(int n, double rate, const double* v, const do
  * d: direction record (rbt_ulayout d_dx, d_da).  steps = {primal, dual}.  (The terminal stage returns 1.0, 1.0 and
  * touches nothing: unconstr_terminal_stage.cpp:97-112 -- the caller skips it.)
  */
-void orc_ustage_expand(int nv, const rbt_constraint_table* tab, double dt, const double* lin, const double* ex,
-                       const double* d, double* con, double* xd, double* steps) {
+void orc_ustage_expand_at(int nv, const rbt_constraint_table* tab, int stage, double dt, const double* lin, const double* ex,
+                          const double* d, double* con, double* xd, double* steps) {
   rbt_ustage_layout S;
   rbt_ulayout K;
   rbt_make_ustage_layout(nv, tab->n_box, &S);
@@ -157,18 +170,19 @@ void orc_ustage_expand(int nv, const rbt_constraint_table* tab, double dt, const
   double* dual = con + S.c_dual;
   for (int r = 0; r < tab->n_box; ++r) {
     const rbt_box_row* b = &tab->box[r];
+    if (!row_acts(b, stage)) continue;
     const double* var = b->var == RBT_VAR_Q ? dq : b->var == RBT_VAR_V ? dv : b->var == RBT_VAR_A ? da : du;
     con[S.c_dslack + r] = -b->sign * var[b->idx] - con[S.c_res + r];
     con[S.c_ddual + r] = -(dual[r] * con[S.c_dslack + r] + con[S.c_cmpl + r]) / slack[r];
   }
-  steps[0] = fraction_to_boundary(tab->n_box, tab->fraction_to_boundary, slack, con + S.c_dslack);
-  steps[1] = fraction_to_boundary(tab->n_box, tab->fraction_to_boundary, dual, con + S.c_ddual);
+  steps[0] = fraction_to_boundary(tab, stage, slack, con + S.c_dslack);
+  steps[1] = fraction_to_boundary(tab, stage, dual, con + S.c_ddual);
 }
 
 /* updatePrimal + updateDual  unconstr_intermediate_stage.cpp:125-144, unconstr_terminal_stage.cpp:115-132,
  * SplitSolution::integrate split_solution.cpp:58-90 (fixed base: q += step*dq). */
-void orc_ustage_update(int nv, const rbt_constraint_table* tab, int terminal, const double* d, const double* xd,
-                       double* con, double* sol, double primal_step, double dual_step) {
+void orc_ustage_update_at(int nv, const rbt_constraint_table* tab, int stage, int terminal, const double* d, const double* xd,
+                          double* con, double* sol, double primal_step, double dual_step) {
   rbt_ustage_layout S;
   rbt_ulayout K;
   rbt_make_ustage_layout(nv, tab->n_box, &S);
@@ -186,9 +200,24 @@ void orc_ustage_update(int nv, const rbt_constraint_table* tab, int terminal, co
     sol[S.s_beta + i] += primal_step * xd[S.x_dbeta + i];
   }
   for (int r = 0; r < tab->n_box; ++r) {
+    if (!row_acts(&tab->box[r], stage)) continue;
     con[S.c_slack + r] += primal_step * con[S.c_dslack + r];
     con[S.c_dual + r] += dual_step * con[S.c_ddual + r];
   }
+}
+
+/* The same three steps on a grid point from stage 2 on, where every row of the table acts. */
+void orc_ustage_condense(int nv, const rbt_constraint_table* tab, int terminal, const double* lin, double* con, double* kkt,
+                         double* ex) {
+  orc_ustage_condense_at(nv, tab, 2, terminal, lin, con, kkt, ex);
+}
+void orc_ustage_expand(int nv, const rbt_constraint_table* tab, double dt, const double* lin, const double* ex, const double* d,
+                       double* con, double* xd, double* steps) {
+  orc_ustage_expand_at(nv, tab, 2, dt, lin, ex, d, con, xd, steps);
+}
+void orc_ustage_update(int nv, const rbt_constraint_table* tab, int terminal, const double* d, const double* xd, double* con,
+                       double* sol, double primal_step, double dual_step) {
+  orc_ustage_update_at(nv, tab, 2, terminal, d, xd, con, sol, primal_step, dual_step);
 }
 
 /* ---------------- batched horizon drivers (UnconstrDirectMultipleShooting::{evalKKT tail, computeStepSizes,
@@ -203,7 +232,7 @@ void orc_ucondense_batch(int nv, const rbt_constraint_table* tab, int N, int bat
   for (int b = 0; b < batch; ++b)
     for (int i = 0; i <= N; ++i) {
       const size_t o = (size_t)b * (N + 1) + i;
-      orc_ustage_condense(nv, tab, i == N, lin + o * S.l_stride, con + o * S.c_stride, kkt + o * K.k_stride, ex + o * S.e_stride);
+      orc_ustage_condense_at(nv, tab, i, i == N, lin + o * S.l_stride, con + o * S.c_stride, kkt + o * K.k_stride, ex + o * S.e_stride);
     }
 }
 
@@ -219,7 +248,7 @@ void orc_uexpand_batch(int nv, const rbt_constraint_table* tab, int N, double dt
     for (int i = 0; i < N; ++i) {
       const size_t o = (size_t)b * (N + 1) + i;
       double st[2];
-      orc_ustage_expand(nv, tab, dt, lin + o * S.l_stride, ex + o * S.e_stride, dir + o * K.d_stride, con + o * S.c_stride,
+      orc_ustage_expand_at(nv, tab, i, dt, lin + o * S.l_stride, ex + o * S.e_stride, dir + o * K.d_stride, con + o * S.c_stride,
                         xd + o * S.x_stride, st);
       if (st[0] < mp) mp = st[0];
       if (st[1] < md) md = st[1];
@@ -239,7 +268,7 @@ void orc_uupdate_batch(int nv, const rbt_constraint_table* tab, int N, int batch
   for (int b = 0; b < batch; ++b)
     for (int i = 0; i <= N; ++i) {
       const size_t o = (size_t)b * (N + 1) + i;
-      orc_ustage_update(nv, tab, i == N, dir + o * K.d_stride, xd + o * S.x_stride, con + o * S.c_stride,
+      orc_ustage_update_at(nv, tab, i, i == N, dir + o * K.d_stride, xd + o * S.x_stride, con + o * S.c_stride,
                         sol + o * S.s_stride, steps[2 * b], steps[2 * b + 1]);
     }
 }

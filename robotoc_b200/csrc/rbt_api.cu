@@ -1686,21 +1686,25 @@ int rbt_unconstr_upload(rbt_uhandle* h, int which, const double* host, void* str
   if (!h || !host) return RBT_ERR_ARG;
   if (which != RBT_BUF_KKT && which != RBT_BUF_DX0 && which != RBT_BUF_LIN && which != RBT_BUF_CON && which != RBT_BUF_SOL)
     return RBT_ERR_ARG;
-  if (!ubuf_ptr(h, which)) {
+  // a table with n_box = 0 has an empty PDIPM record: its buffer is a null allocation, and copying it is a no-op
+  const long long n = rbt_unconstr_buf_doubles(h, which);
+  if (n < 0 || (n > 0 && !ubuf_ptr(h, which))) {
     h->err = "rbt_unconstr_upload: stage layer not set up (rbt_unconstr_stage_setup)";
     return RBT_ERR_STATE;
   }
+  if (n == 0) return RBT_OK;
   RBT_CUDA(h, cudaSetDevice(h->device));
-  RBT_CUDA(h, cudaMemcpyAsync(ubuf_ptr(h, which), host, size_t(rbt_unconstr_buf_doubles(h, which)) * 8,
-                              cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  RBT_CUDA(h, cudaMemcpyAsync(ubuf_ptr(h, which), host, size_t(n) * 8, cudaMemcpyHostToDevice, (cudaStream_t)stream));
   return RBT_OK;
 }
 
 int rbt_unconstr_download(rbt_uhandle* h, int which, double* host, void* stream) {
-  if (!h || !host || !ubuf_ptr(h, which)) return RBT_ERR_ARG;
+  if (!h || !host) return RBT_ERR_ARG;
+  const long long n = rbt_unconstr_buf_doubles(h, which);
+  if (n < 0 || (n > 0 && !ubuf_ptr(h, which))) return RBT_ERR_ARG;
+  if (n == 0) return RBT_OK;
   RBT_CUDA(h, cudaSetDevice(h->device));
-  RBT_CUDA(h, cudaMemcpyAsync(host, ubuf_ptr(h, which), size_t(rbt_unconstr_buf_doubles(h, which)) * 8,
-                              cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  RBT_CUDA(h, cudaMemcpyAsync(host, ubuf_ptr(h, which), size_t(n) * 8, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return RBT_OK;
 }
 

@@ -13,6 +13,12 @@
 // one (OCP, stage) pair; the linearization record is pulled into shared memory with coalesced loads, everything is done
 // in place there, and the KKT / expansion records leave with coalesced stores.  No tensor cores: nothing here reaches
 // an 8x8x4 DMMA tile without padding 7 -> 8, and the kernel is bound by the record traffic anyway.
+//
+// Joint limits act from the grid point the reference gives them: UnconstrOCPSolver sets GridInfo::stage = i, and
+// ConstraintsData::setTimeStage (src/constraints/constraints_data.cpp:20-45) turns the position level off on stages 0 and 1
+// and the velocity level off on stage 0.  A row of level urow_level(var) acts on grid point i iff i >= that level; a row
+// that does not act adds nothing to the KKT / expansion records, takes no part in the step sizes, and its PDIPM record is
+// left untouched.
 #pragma once
 #include "rbt_device.cuh"
 #include "stage_kernels.cuh"  // warp_min, atomic_min_pos
@@ -35,6 +41,8 @@ struct UStageParams {
   double* sol;
   double* steps;
 };
+
+__device__ __forceinline__ int urow_level(int var) { return var == RBT_VAR_Q ? 2 : var == RBT_VAR_V ? 1 : 0; }
 
 template <int NV>
 struct UStageCfg {
@@ -97,13 +105,14 @@ __global__ void __launch_bounds__(32 * UStageCfg<NV>::WARPS) ucondense_kernel(co
   // ---- PDIPM rows: cmpl, cond per row (parallel), then one lane per target variable gathers its rows in table order
   const int nbox = p.tab.n_box;
   for (int r = lane; r < nbox; r += 32) {
+    if (i < urow_level(p.tab.box[r].var)) continue;
     const double sl = con[S.c_slack + r], du = con[S.c_dual + r], rs = con[S.c_res + r];
     const double cm = sl * du - p.tab.barrier;
     con[S.c_cmpl + r] = cm;
     con[S.c_cond + r] = (du * rs - cm) / sl;
   }
   __syncwarp();
-  if (lane < 4 * NV) {
+  if (lane < 4 * NV && i >= urow_level(lane / NV)) {
     const int var = lane / NV, idx = lane % NV;
     double dacc = 0.0, gacc = 0.0;
     double* dptr = var == RBT_VAR_Q ? &Qxx[idx + idx * NX] : var == RBT_VAR_V ? &Qxx[(NV + idx) * (NX + 1)]
@@ -221,6 +230,7 @@ __global__ void __launch_bounds__(128) uexpand_kernel(const UStageParams p) {
   const double rate = p.tab.fraction_to_boundary;
   for (int r = lane; r < p.tab.n_box; r += 32) {
     const rbt_box_row br = p.tab.box[r];
+    if (i < urow_level(br.var)) continue;
     const double* var = br.var == RBT_VAR_Q ? dx : br.var == RBT_VAR_V ? dx + NV : br.var == RBT_VAR_A ? da : du;
     const double sl = con[S.c_slack + r], dl = con[S.c_dual + r];
     const double ds = -br.sign * var[br.idx] - con[S.c_res + r];
@@ -266,6 +276,7 @@ __global__ void __launch_bounds__(128) uupdate_kernel(const UStageParams p) {
   }
   if (terminal) return;
   for (int r = lane; r < p.tab.n_box; r += 32) {
+    if (i < urow_level(p.tab.box[r].var)) continue;
     con[S.c_slack + r] += ps * con[S.c_dslack + r];
     con[S.c_dual + r] += ds * con[S.c_ddual + r];
   }

@@ -314,3 +314,33 @@ def rel_err(a, b):
     a, b = np.asarray(a), np.asarray(b)
     denom = max(np.max(np.abs(b)), 1e-300)
     return float(np.max(np.abs(a - b)) / denom)
+
+
+def unconstr_step_coverage(S, tab, N, con, out, dx0, binds, gated):
+    """Asserts what a step-size case of the unconstrained path reaches (out: oracle_lib.unconstr_iteration of the inputs con,
+    dx0): primal and dual steps of every OCP below 1 and different; the primal / dual minimum of every OCP at the (grid
+    point, row) `binds` names for it; and every `gated` (b, 0, r) position row on grid 0 would bind at a tenth of the step or
+    less if it were counted, while it takes no part (its dslack stays as it came in)."""
+    from robotoc_b200.stage import VAR_Q, VAR_V
+    nb = tab.n_box
+    level = np.array([2 if tab.box[r].var == VAR_Q else 1 if tab.box[r].var == VAR_V else 0 for r in range(nb)])
+    steps = out["steps"]
+    assert (steps < 1).all() and (steps[:, 0] != steps[:, 1]).all(), steps
+    for b, i, r, kind in binds:
+        fr = np.full((N, nb), np.inf)
+        for g in range(N):
+            c = out["con_expanded"][b, g]
+            v, dv = (c[S.c_slack:S.c_slack + nb], c[S.c_dslack:S.c_dslack + nb]) if kind == "p" else \
+                (c[S.c_dual:S.c_dual + nb], c[S.c_ddual:S.c_ddual + nb])
+            with np.errstate(divide="ignore", invalid="ignore"):
+                f = -tab.fraction_to_boundary * (v / dv)
+            fr[g] = np.where((g >= level) & (f > 0) & (f < 1), f, np.inf)
+        assert np.unravel_index(np.argmin(fr), fr.shape) == (i, r), (b, i, r, kind)
+        assert fr.min() == steps[b, 0 if kind == "p" else 1]
+    for b, i, r in gated:
+        assert i == 0 and level[r] == 2
+        bx = tab.box[r]
+        ds = -bx.sign * dx0[b, bx.idx] - con[b, 0, S.c_res + r]
+        would = -tab.fraction_to_boundary * con[b, 0, S.c_slack + r] / ds
+        assert 0 < would < 0.1 * steps[b, 0], (would, steps[b, 0])
+        assert out["con_expanded"][b, 0, S.c_dslack + r] == con[b, 0, S.c_dslack + r]

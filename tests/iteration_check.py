@@ -314,3 +314,47 @@ def oracle_trials(lib, sd, table, ctrl, sol, ref, n_trials, rate=0.75):
                         P(ref["cc_exp"]), P(ref["steps"]), P(alphas), P(trial), P(barrier))
     return alphas, barrier, trial
 
+
+
+def unconstr_blocks(S, UL):
+    """(record key, block name, offset, size) of every block of the unconstrained iteration's records, grouped by family."""
+    nv, nx, nb = S.nv, S.nx, S.nbox
+    kkt = [("kkt", "Qxx", UL.k_Qxx, nx * nx), ("kkt", "Qxu", UL.k_Qxu, nx * nv), ("kkt", "Qaa", UL.k_Qaa, nv * nv),
+           ("kkt", "Fx", UL.k_Fx, nx), ("kkt", "lx", UL.k_lx, nx), ("kkt", "la", UL.k_la, nv)]
+    ex = [("ex", "lu", S.e_lu, nv), ("ex", "Quu", S.e_Quu, nv * nv)]
+    pdipm = [(k, f, getattr(S, "c_" + f), nb) for k, fs in (("con_condensed", ("cmpl", "cond")),
+                                                               ("con_expanded", ("dslack", "ddual")),
+                                                               ("con", ("slack", "dual", "res", "cmpl", "cond", "dslack", "ddual")))
+             for f in fs]
+    xd = [("xd", "du", S.x_du, nv), ("xd", "dbeta", S.x_dbeta, nv)]
+    d = [("dir", "dx", UL.d_dx, nx), ("dir", "dlmdgmm", UL.d_dlmdgmm, nx), ("dir", "da", UL.d_da, nv)]
+    sol = [("sol", f, getattr(S, "s_" + f), nv) for f in ("q", "v", "a", "u", "beta", "lmd", "gmm")]
+    return {"kkt": kkt, "expansion": ex, "pdipm": pdipm, "expanded direction": xd, "direction": d, "solution": sol}
+
+
+def compare_unconstr_records(S, UL, got, ref, tol, ocps=None):
+    """Every block of every record of the unconstrained iteration (oracle_lib / ref_lib.unconstr_iteration dictionaries), on
+    every grid point of every OCP, relative to that block's own scale there: max |got - ref| / max |ref| (an all-zero reference
+    block must come out exactly zero).  The step sizes are compared whole.  ocps: the OCPs to compare (default all).
+    Returns the worst error per block family."""
+    worst = {}
+    sel = slice(None) if ocps is None else list(ocps)
+    for fam, blocks in unconstr_blocks(S, UL).items():
+        w = 0.0
+        for key, name, off, n in blocks:
+            if n == 0:  # a table without rows
+                continue
+            g, r = np.asarray(got[key])[sel][..., off:off + n], np.asarray(ref[key])[sel][..., off:off + n]
+            scale = np.abs(r).max(axis=-1)
+            err = np.abs(g - r).max(axis=-1) / np.where(scale > 0, scale, 1e-300)
+            err = np.where(np.isnan(err), np.inf, err)
+            if err.size and err.max() > tol:
+                b, i = np.unravel_index(np.argmax(err), err.shape)
+                raise AssertionError(f"{key}.{name}: OCP {b}, grid point {i}: relative error {err.max():.3e} > {tol:.1e}")
+            w = max(w, float(err.max()) if err.size else 0.0)
+        worst[fam] = w
+    g, r = np.asarray(got["steps"])[sel], np.asarray(ref["steps"])[sel]
+    err = float(np.max(np.abs(g - r) / np.abs(r)))
+    assert err <= tol, f"steps: relative error {err:.3e} > {tol:.1e}"
+    worst["steps"] = err
+    return worst

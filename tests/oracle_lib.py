@@ -55,6 +55,8 @@ def load():
     L.orc_ustage_expand.restype = None
     L.orc_ustage_update.argtypes = [c_int, ptab, c_int, c_vp, c_vp, c_vp, c_vp, c_dbl, c_dbl]
     L.orc_ustage_update.restype = None
+    L.orc_ustage_condense_at.argtypes = [c_int, ptab, c_int, c_int, c_vp, c_vp, c_vp, c_vp]
+    L.orc_ustage_condense_at.restype = None
     L.orc_ucondense_batch.argtypes = [c_int, ptab, c_int, c_int, c_vp, c_vp, c_vp, c_vp]
     L.orc_ucondense_batch.restype = None
     L.orc_uexpand_batch.argtypes = [c_int, ptab, c_int, c_dbl, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]

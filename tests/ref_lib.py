@@ -137,6 +137,51 @@ def reference_iteration(sd, S, K, table, ctrl, lin, con, dx0):
                 cc_upd=cc_upd, ex_upd=ex_upd, perf_stage=perf_stage)
 
 
+def unconstr_iteration(nv, UL, S, tab, N, dt, lin, con, sol, dx0):
+    """One hot-path iteration of the unconstrained (fixed-base) path computed by the REFERENCE's own code: stage-layer
+    condensing on every grid point (ref_ustage phase 1, oracle/ref_wrap/ref_ustage_wrap.cpp) -> robotoc::UnconstrRiccatiRecursion
+    (ref_unconstr_batch) -> expansion and step sizes (phase 2) -> horizon minimum -> solution, slack and dual update (phase 3).
+    Same record dictionary as oracle_lib.unconstr_iteration (minus `ric`, `info`)."""
+    lib = load()
+    if not hasattr(lib, "_ustage_ready"):
+        c_int, c_dbl, c_vp = ctypes.c_int, ctypes.c_double, ctypes.c_void_p
+        lib.ref_ustage.argtypes = [c_int, c_vp, c_int, c_int, c_dbl] + [c_vp] * 8 + [c_dbl, c_dbl, c_int]
+        lib._ustage_ready = True
+    batch = lin.shape[0]
+    kkt = np.zeros((batch, N + 1, UL.k_stride))
+    ex = np.zeros((batch, N + 1, S.e_stride))
+    con_c, con_e, con_u = con.copy(), con.copy(), con.copy()
+    xd = np.zeros((batch, N + 1, S.x_stride))
+    sol_u = sol.copy()
+    steps = np.ones((batch, 2))
+    zero_d = np.zeros(UL.d_stride)
+
+    def run(b, i, d, phase, alpha, c_out, kkt_out, ex_out, xd_out, sol_out):
+        c = con[b, i].copy()
+        k, e, x, s = np.zeros(UL.k_stride), np.zeros(S.e_stride), np.zeros(S.x_stride), sol[b, i].copy()
+        st = np.ones(2)
+        rc = lib.ref_ustage(nv, ctypes.byref(tab), i, N, dt, _ptr(np.ascontiguousarray(lin[b, i])), _ptr(c), _ptr(k), _ptr(e),
+                            _ptr(np.ascontiguousarray(d)), _ptr(x), _ptr(s), _ptr(st), alpha[0], alpha[1], phase)
+        assert rc == 0, "the reference cannot express this constraint table"
+        c_out[b, i] = c
+        for out, v in ((kkt_out, k), (ex_out, e), (xd_out, x), (sol_out, s)):
+            if out is not None:
+                out[b, i] = v
+        return st
+
+    for b in range(batch):
+        for i in range(N + 1):
+            run(b, i, zero_d, 1, (1.0, 1.0), con_c, kkt, ex, None, None)
+    _, _, d = unconstr_batch(nv, UL, N, dt, kkt, dx0)
+    for b in range(batch):
+        for i in range(N):
+            steps[b] = np.minimum(steps[b], run(b, i, d[b, i], 2, (1.0, 1.0), con_e, None, None, xd, None))
+    for b in range(batch):
+        for i in range(N + 1):
+            run(b, i, d[b, i], 3, steps[b], con_u, None, None, None, sol_u)
+    return dict(kkt=kkt, ex=ex, con_condensed=con_c, dir=d, xd=xd, steps=steps, con_expanded=con_e, con=con_u, sol=sol_u)
+
+
 LIB_DISCRETIZE = os.path.join(ORACLE_DIR, "_ref", "libref_discretize.so")
 _lib_td = None
 

@@ -330,3 +330,41 @@ def make_unconstr_stage_inputs(S, N: int, batch: int, seed: int):
         con[:, i, S.c_res:S.c_res + nb] = 0.1 * u(batch, nb)
     dx0 = 0.1 * u(batch, nx)
     return np.ascontiguousarray(lin), np.ascontiguousarray(con), np.ascontiguousarray(sol), np.ascontiguousarray(dx0)
+
+
+def unconstr_table(rows, barrier=1.0e-3, fraction_to_boundary=0.995):
+    """rbt_constraint_table for the unconstrained path (n_contacts = 0) with the box rows `rows` = [(var, idx, sign), ...], in
+    that order."""
+    from robotoc_b200.stage import rbt_constraint_table
+    t = rbt_constraint_table()
+    t.n_contacts = 0
+    t.barrier, t.fraction_to_boundary = barrier, fraction_to_boundary
+    for r, (var, idx, sign) in enumerate(rows):
+        t.box[r].var, t.box[r].idx, t.box[r].sign = var, idx, sign
+    t.n_box = len(rows)
+    return t
+
+
+def table_rows(tab):
+    return [(tab.box[r].var, tab.box[r].idx, tab.box[r].sign) for r in range(tab.n_box)]
+
+
+def iiwa14_rows(nv=7, acceleration_limits=False):
+    """Box rows of examples/iiwa14/unconstr_ocp_benchmark.cpp:45-60 in component order (joint position, velocity, torque
+    lower / upper limits), optionally followed by JointAccelerationLowerLimit / UpperLimit: what the reference can express."""
+    from robotoc_b200.stage import VAR_A, VAR_Q, VAR_U, VAR_V
+    vs = (VAR_Q, VAR_V, VAR_U) + ((VAR_A,) if acceleration_limits else ())
+    return [(var, j, sign) for var in vs for sign in (-1, +1) for j in range(nv)]
+
+
+def bind_unconstr_rows(S, con, binds, R=(100.0, 50.0)):
+    """Makes chosen rows the binding rows of the fraction-to-boundary rule.  binds: [(b, i, r, kind)], kind "p" (primal: the
+    Newton step drives the slack of row r on grid point i of OCP b far below zero) or "d" (dual: the slack grows by far more
+    than it is, which drives the dual below zero).  slack = dual = 1e-4 keeps the row's barrier weight near the cost
+    curvature, so the condensed step cannot satisfy the linearised row; the residual R sets how far it misses."""
+    con = con.copy()
+    for b, i, r, kind in binds:
+        con[b, i, S.c_slack + r] = 1.0e-4
+        con[b, i, S.c_dual + r] = 1.0e-4
+        con[b, i, S.c_res + r] = R[0] if kind == "p" else -R[1]
+    return con

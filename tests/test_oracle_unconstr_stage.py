@@ -5,6 +5,7 @@ test/dynamics/unconstr_dynamics_test.cpp (condense vs explicit block formulas)."
 import ctypes
 
 import numpy as np
+import pytest
 
 import oracle_lib
 from oracle_lib import ptr
@@ -36,6 +37,12 @@ def _jac(tab):
     return J
 
 
+def _acts(tab, stage):
+    """Rows that act on grid point `stage` (ConstraintsData::setTimeStage, constraints_data.cpp:20-45): position rows from
+    stage 2, velocity rows from stage 1, acceleration and torque rows everywhere."""
+    return np.array([stage >= {VAR_Q: 2, VAR_V: 1}.get(tab.box[r].var, 0) for r in range(tab.n_box)])
+
+
 def test_layout_matches_header_rules():
     tab = iiwa14_constraint_table()
     lib, S, UL = _layouts(tab)
@@ -46,18 +53,33 @@ def test_layout_matches_header_rules():
 
 
 def test_condensed_model_equals_substituted_model():
+    _check_condensed_model(2)
+
+
+@pytest.mark.parametrize("stage", [0, 1])
+def test_condensed_model_on_grid_points_0_and_1_carries_only_the_rows_that_act(stage):
+    """Grid point 0 carries the torque and acceleration rows, grid point 1 also the velocity rows; the PDIPM records of the
+    other rows are left as they came in."""
+    _check_condensed_model(stage)
+
+
+def _check_condensed_model(stage):
     tab = iiwa14_constraint_table()
     tab.box[5].var = VAR_A  # make sure an acceleration row is exercised too
     lib, S, UL = _layouts(tab)
     lin, con, sol, dx0 = make_unconstr_stage_inputs(S, 1, 4, seed=5)
     nx = 2 * NV
+    act = _acts(tab, stage)
+    assert act.sum() == {0: 15, 1: 29, 2: 42}[stage]
     for b in range(4):
         l, c = lin[b, 0].copy(), con[b, 0].copy()
+        c[S.c_cmpl:S.c_cmpl + tab.n_box] = c[S.c_cond:S.c_cond + tab.n_box] = np.nan  # rows that do not act stay untouched
+        c_in = c.copy()
         kkt, ex = np.zeros(UL.k_stride), np.zeros(S.e_stride)
-        lib.orc_ustage_condense(NV, ctypes.byref(tab), 0, ptr(l), ptr(c), ptr(kkt), ptr(ex))
-        # full model over z = (q, v, a, u) after the PDIPM terms
-        slack, dual, res = (con[b, 0, o:o + tab.n_box] for o in (S.c_slack, S.c_dual, S.c_res))
-        J = _jac(tab)
+        lib.orc_ustage_condense_at(NV, ctypes.byref(tab), stage, 0, ptr(l), ptr(c), ptr(kkt), ptr(ex))
+        # full model over z = (q, v, a, u) after the PDIPM terms of the rows that act
+        slack, dual, res = (con[b, 0, o:o + tab.n_box][act] for o in (S.c_slack, S.c_dual, S.c_res))
+        J = _jac(tab)[act]
         cmpl = slack * dual - tab.barrier
         cond = (dual * res - cmpl) / slack
         H = np.zeros((4 * NV, 4 * NV))
@@ -67,8 +89,12 @@ def test_condensed_model_equals_substituted_model():
         g = np.concatenate([l[S.l_lx:S.l_lx + nx], l[S.l_la:S.l_la + NV], l[S.l_lu:S.l_lu + NV]])
         H += J.T @ np.diag(dual / slack) @ J
         g += J.T @ cond
-        np.testing.assert_allclose(c[S.c_cmpl:S.c_cmpl + tab.n_box], cmpl, rtol=1e-14)
-        np.testing.assert_allclose(c[S.c_cond:S.c_cond + tab.n_box], cond, rtol=1e-13)
+        np.testing.assert_allclose(c[S.c_cmpl:S.c_cmpl + tab.n_box][act], cmpl, rtol=1e-14)
+        np.testing.assert_allclose(c[S.c_cond:S.c_cond + tab.n_box][act], cond, rtol=1e-13)
+        for o in (S.c_cmpl, S.c_cond):
+            np.testing.assert_array_equal(c[o:o + tab.n_box][~act], c_in[o:o + tab.n_box][~act])
+        np.testing.assert_array_equal(np.delete(c, np.r_[S.c_cmpl:S.c_cmpl + tab.n_box, S.c_cond:S.c_cond + tab.n_box]),
+                                      np.delete(c_in, np.r_[S.c_cmpl:S.c_cmpl + tab.n_box, S.c_cond:S.c_cond + tab.n_box]))
         # substitute du = ID + D y, y = (dq, dv, da)
         D = np.hstack([_m(l, S.l_dIDdq, NV, NV), _m(l, S.l_dIDdv, NV, NV), _m(l, S.l_dIDda, NV, NV)])
         ID = l[S.l_ID:S.l_ID + NV]
@@ -122,7 +148,9 @@ def test_terminal_stage_copies_cost_only():
 
 
 def test_expand_update_consistency():
-    """One full iteration on the oracle; the expanded step satisfies the linearised stage equations it was eliminated from."""
+    """One full iteration on the oracle; the expanded step satisfies the linearised stage equations it was eliminated from, on
+    the rows that act on each grid point; the PDIPM records of the rows that do not act (position rows on grid points 0 and 1,
+    velocity rows on grid point 0) come out bit-unchanged, and those rows take no part in the step sizes."""
     tab = iiwa14_constraint_table()
     lib, S, UL = _layouts(tab)
     N, dt, batch = 6, 0.05, 3
@@ -141,19 +169,23 @@ def test_expand_update_consistency():
             # stationarity w.r.t. u of the stage Lagrangian: lu' + Quu' du - dt*dbeta = 0   (linearizeUnconstrDynamics :62)
             dbeta = xd[S.x_dbeta:S.x_dbeta + NV]
             np.testing.assert_allclose(ex[S.e_lu:S.e_lu + NV] + _m(ex, S.e_Quu, NV, NV) @ du - dt * dbeta, 0, atol=1e-11)
+            act = _acts(tab, i)
+            for rec in (out["con_condensed"], out["con_expanded"], out["con"]):
+                rows = lambda c: c[:7 * S.ncp].reshape(7, S.ncp)[:, :nb][:, ~act]  # noqa: E731  (slack ... ddual)
+                np.testing.assert_array_equal(rows(rec[b, i]), rows(con[b, i]))
             c0, c1 = out["con_condensed"][b, i], out["con_expanded"][b, i]
-            slack, dual, res, cmpl = (c0[o:o + nb] for o in (S.c_slack, S.c_dual, S.c_res, S.c_cmpl))
-            dslack, ddual = c1[S.c_dslack:S.c_dslack + nb], c1[S.c_ddual:S.c_ddual + nb]
+            slack, dual, res, cmpl = (c0[o:o + nb][act] for o in (S.c_slack, S.c_dual, S.c_res, S.c_cmpl))
+            dslack, ddual = c1[S.c_dslack:S.c_dslack + nb][act], c1[S.c_ddual:S.c_ddual + nb][act]
             z = np.concatenate([dq, dv, da, du])
-            np.testing.assert_allclose(J @ z + dslack + res, 0, atol=1e-12)            # linearised g + slack = 0
+            np.testing.assert_allclose(J[act] @ z + dslack + res, 0, atol=1e-12)            # linearised g + slack = 0
             np.testing.assert_allclose(slack * ddual + dual * dslack + cmpl, 0, atol=1e-12)  # linearised complementarity
             fp = -tab.fraction_to_boundary * (slack / dslack)
             fd = -tab.fraction_to_boundary * (dual / ddual)
             mins_p.append(min([1.0] + [f for f in fp if 0 < f < 1]))
             mins_d.append(min([1.0] + [f for f in fd if 0 < f < 1]))
             ps, ds = out["steps"][b]
-            np.testing.assert_allclose(out["con"][b, i, S.c_slack:S.c_slack + nb], slack + ps * dslack, rtol=1e-14)
-            np.testing.assert_allclose(out["con"][b, i, S.c_dual:S.c_dual + nb], dual + ds * ddual, rtol=1e-14)
+            np.testing.assert_allclose(out["con"][b, i, S.c_slack:S.c_slack + nb][act], slack + ps * dslack, rtol=1e-14)
+            np.testing.assert_allclose(out["con"][b, i, S.c_dual:S.c_dual + nb][act], dual + ds * ddual, rtol=1e-14)
             assert (out["con"][b, i, S.c_slack:S.c_slack + nb] > 0).all() and (out["con"][b, i, S.c_dual:S.c_dual + nb] > 0).all()
             for off, dd in ((S.s_q, dq), (S.s_v, dv), (S.s_a, da), (S.s_u, du), (S.s_beta, dbeta)):
                 np.testing.assert_allclose(out["sol"][b, i, off:off + NV], sol[b, i, off:off + NV] + ps * dd, rtol=1e-13, atol=1e-14)
