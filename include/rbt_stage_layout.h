@@ -189,6 +189,9 @@ enum { RBT_COST_GENERAL = 0, RBT_COST_ROBOTOC = 1 };
 /* OR-ed into cost_structure: the device fills the inverse-dynamics rows (rbt_linearize_inverse_dynamics), so non-terminal wire
  * records carry neither M nor the first nv rows of dIDCdqv and IDC -- only their nf contact rows */
 #define RBT_WIRE_DEVICE_ID 2
+/* OR-ed into cost_structure: the device fills the contact rows (rbt_linearize_contact_kinematics), so non-terminal wire records
+ * carry neither J nor the nf contact rows of dIDCdqv and IDC; alone or together with RBT_WIRE_DEVICE_ID */
+#define RBT_WIRE_DEVICE_CONTACT 4
 #define RBT_WIRE_MAX_SEGS 20
 #define RBT_WIRE_MAX_ZERO 5
 typedef struct rbt_wire_layout {
@@ -221,6 +224,7 @@ static inline RBT_HD void rbt_make_wire_layout(const rbt_stage_layout* L, const 
                                                rbt_wire_layout* W) {
   const int nv = L->nv, nx = L->nx, nf = c->nf, nvf = nv + nf;
   const int dc = ((cost_structure & RBT_COST_ROBOTOC) != 0), did = ((cost_structure & RBT_WIRE_DEVICE_ID) != 0);
+  const int dcon = ((cost_structure & RBT_WIRE_DEVICE_CONTACT) != 0);
   int ci;
   cost_structure &= RBT_COST_ROBOTOC;
   W->nseg = 0; W->nzero = 0; W->w_doubles = 0; W->ocp_off = 0;
@@ -230,12 +234,16 @@ static inline RBT_HD void rbt_make_wire_layout(const rbt_stage_layout* L, const 
     rbt_wire_add_(W, L->l_se3 + 36, 36, 1, 36, 0);
     return;
   }
-  if (!did) {
+  if (!did && dcon) {  /* ID rows only: M, [dIDdq | dIDdv], ID */
+    rbt_wire_add_(W, L->l_M, nv, nv, nv, 1);
+    rbt_wire_add_(W, L->l_D, nv, nx, L->nvf, 0);
+    rbt_wire_add_(W, L->l_IDC, nv, 1, nv, 0);
+  } else if (!did) {
     rbt_wire_add_(W, L->l_M, nv, nv, nv, 1);
     if (nf > 0) rbt_wire_add_(W, L->l_J, nf, nv, L->nfm, 0);
     rbt_wire_add_(W, L->l_D, nvf, nx, L->nvf, 0);
     rbt_wire_add_(W, L->l_IDC, nvf, 1, nvf, 0);
-  } else if (nf > 0) {  /* contact rows only: dCda, [dCdq | dCdv], C */
+  } else if (nf > 0 && !dcon) {  /* contact rows only: dCda, [dCdq | dCdv], C */
     rbt_wire_add_(W, L->l_J, nf, nv, L->nfm, 0);
     rbt_wire_add_(W, L->l_D + nv, nf, nx, L->nvf, 0);
     rbt_wire_add_(W, L->l_IDC + nv, nf, 1, nf, 0);

@@ -49,8 +49,10 @@ enum {
   RBT_BUF_SOL = 9,   /* solution records (q, v, a, dv, u, f, lmd, gmm, beta, mu, nu_passive, xi), updated in place */
   RBT_BUF_XDIR = 10, /* expanded direction records (daf, dbetamu, dnu_passive) */
   RBT_BUF_STEPS = 11,/* [batch][2] max primal / dual step size over the horizon */
-  RBT_BUF_PERF = 12  /* [batch][8] PerformanceIndex of rbt_eval_kkt: {cost (0: not evaluated on this path), cost_barrier,
+  RBT_BUF_PERF = 12, /* [batch][8] PerformanceIndex of rbt_eval_kkt: {cost (0: not evaluated on this path), cost_barrier,
                         primal_feasibility, dual_feasibility, kkt_error, sqrt(kkt_error) = OCPSolver::KKTError(), 0, 0} */
+  RBT_BUF_CONTACT_POS = 13  /* [batch][n_grid][n_contacts][3] desired contact positions of rbt_linearize_contact_kinematics
+                               (ContactStatus::contactPosition of each grid point's phase); allocated by its first upload */
 };
 
 typedef struct rbt_handle rbt_handle;
@@ -220,6 +222,27 @@ int rbt_set_robot_model(rbt_handle* h, const rbt_robot_model* model);
  * rbt_eval_kkt / rbt_condense; the uploaded records' ID sections are ignored and their gradients lack the beta terms.
  * RBT_ERR_STATE before rbt_set_robot_model. */
 int rbt_linearize_inverse_dynamics(rbt_handle* h, void* stream);
+/* Baumgarte gains of the point contacts (SURVEY.md 8f-1, second slice): gains_host[n_contacts][2] = {baumgarte_position_gain,
+ * baumgarte_velocity_gain} of ContactModelInfo (include/robotoc/robot/contact_model_info.hpp), as each PointContact holds them
+ * (point_contact.hxx:29-33).  RBT_ERR_ARG if a gain is negative or not finite (PointContact's constructor throws,
+ * src/robot/point_contact.cpp:27-34); RBT_ERR_STATE before rbt_stage_setup. */
+int rbt_set_contact_gains(rbt_handle* h, const double* gains_host);
+/* The contact rows of linearizeContactDynamics (src/dynamics/contact_dynamics.cpp:12-52: Robot::computeBaumgarteResidual /
+ * computeBaumgarteDerivatives, robot.hxx:291-360, PointContact, point_contact.hxx:16-86) on Intermediate and Lift grid points,
+ * kinematics at (q, v, a) without gravity (intermediate_stage.cpp:94), and of linearizeImpactDynamics (impact_dynamics.cpp:8-35:
+ * computeImpactVelocityResidual / Derivatives, point_contact.hxx:89-117) on Impact grid points, kinematics at (q, v + dv)
+ * (impact_stage.cpp:61,89).  Per active point contact, in contact order, three rows:
+ *   Intermediate / Lift: C = a_cl + kv v_f,lin + kp (oMf.p - p_des) with a_cl = a_f,lin + w_f x v_f,lin (LOCAL frame),
+ *                        p_des from RBT_BUF_CONTACT_POS; J = dC/da = J_lin; [dC/dq | dC/dv];
+ *   Impact:              C = v_f,lin; J = dC/dv = J_lin; [dv_f,lin/dq | J_lin].
+ * Writes J (ld nf_max), rows nv .. nv+nf-1 of dIDCdqv and of IDC into RBT_BUF_LIN, full width, and updates the gradients:
+ * lf -= J beta, lq += dCdq^T mu, lv += dCdv^T mu, la (impact: ldv) += J^T mu (contact_dynamics.cpp:34-36,47-51,
+ * impact_dynamics.cpp:27-31).  Derivatives in q in the tangent space, as rbt_linearize_inverse_dynamics.  Inactive rows,
+ * grid points without contacts, terminal grid points and every other section are untouched.
+ * Order: rbt_upload(LIN, CON, SOL) -> (rbt_linearize_joint_limits) -> (rbt_linearize_inverse_dynamics) ->
+ * rbt_linearize_contact_kinematics -> rbt_eval_kkt / rbt_condense.  RBT_ERR_STATE until rbt_set_robot_model,
+ * rbt_set_contact_gains and one rbt_upload(RBT_BUF_CONTACT_POS) have been made. */
+int rbt_linearize_contact_kinematics(rbt_handle* h, void* stream);
 /* computeInitialStateDirection (src/dynamics/state_equation.cpp:98-109) into RBT_BUF_DX0.  dq0_v0_host: [batch][2 nv] =
  * {q0 (-) s[0].q from Robot::subtractConfiguration (the robot model stays on the host), v0}; uses the stage-0 Fqq_prev_inv that
  * rbt_condense left in RBT_BUF_EXP and s[0].v of RBT_BUF_SOL, so call it after rbt_condense and before rbt_riccati_forward. */
@@ -294,7 +317,10 @@ int rbt_iteration_host_resident(rbt_handle* h, const double* wire_host, const do
  * RBT_WIRE_DEVICE_ID OR-ed into cost_structure (rbt_stage_layout.h): the device computes the inverse-dynamics rows
  * (rbt_linearize_inverse_dynamics, after rbt_set_robot_model), so the wire records drop M, the ID rows of dIDCdqv and of IDC,
  * and their gradients lack the beta terms; rbt_iteration_host_wire / _resident run the kernel right after the unpack and
- * rbt_iteration_host_bytes counts the smaller records. */
+ * rbt_iteration_host_bytes counts the smaller records.  RBT_WIRE_DEVICE_CONTACT, alone or with RBT_WIRE_DEVICE_ID: the device
+ * computes the contact rows (rbt_linearize_contact_kinematics, after rbt_set_robot_model, rbt_set_contact_gains and an upload of
+ * RBT_BUF_CONTACT_POS), so the records drop J and the contact rows of dIDCdqv and IDC and their gradients lack the multiplier
+ * terms of the contact rows; the kernel runs right after the inverse-dynamics kernel (or the unpack). */
 int rbt_set_wire_cost_structure(rbt_handle* h, int cost_structure);
 int rbt_wire_doubles(const rbt_stage_dims* sdims, const rbt_stage_ctrl* ctrl, int n_grid, int cost_structure);   /* doubles per OCP */
 int rbt_wire_layout_get(const rbt_stage_dims* sdims, const rbt_stage_ctrl* ctrl, int n_grid, int cost_structure, int i,

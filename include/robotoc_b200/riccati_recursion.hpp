@@ -425,10 +425,39 @@ class DirectMultipleShooting {
     rr_.check(rbt_download(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
     rr_.check(rbt_sync(rr_.handle(), nullptr));
   }
+  /// Baumgarte gains of the point contacts, [n_contacts][2] = {baumgarte_position_gain, baumgarte_velocity_gain} of
+  /// ContactModelInfo (rbt_set_contact_gains; INTEGRATION.md 5b).
+  void setContactGains(const std::vector<double>& gains) {
+    if (gains.size() != size_t(2) * sdims_.n_contacts)
+      throw std::invalid_argument("[DirectMultipleShooting] invalid argument: gains must hold 2 values per contact");
+    rr_.check(rbt_set_contact_gains(rr_.handle(), gains.data()));
+  }
+  /// Desired contact positions [batch][n_grid][n_contacts][3] (ContactStatus::contactPosition of each grid point's phase),
+  /// uploaded to RBT_BUF_CONTACT_POS; they stay on the device until the next call.
+  void setContactPositions(const std::vector<double>& pos) {
+    if (pos.size() != size_t(rr_.batch()) * rr_.n_grid() * sdims_.n_contacts * 3)
+      throw std::invalid_argument("[DirectMultipleShooting] invalid argument: contact positions must be [batch][n_grid][n_contacts][3]");
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_CONTACT_POS, pos.data(), nullptr));
+    rr_.check(rbt_sync(rr_.handle(), nullptr));
+  }
+  /// The contact rows of linearizeContactDynamics / linearizeImpactDynamics on the device (rbt_linearize_contact_kinematics):
+  /// `lin` and `sol` are uploaded, `lin` is read back with J, the contact rows of dIDCdqv / IDC and the multiplier terms of the
+  /// gradients filled in.
+  void linearizeContactKinematics(std::vector<double>& lin, const std::vector<double>& sol) {
+    expect(lin, S_.l_stride, "lin");
+    expect(sol, S_.s_stride, "sol");
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_SOL, sol.data(), nullptr));
+    rr_.check(rbt_linearize_contact_kinematics(rr_.handle(), nullptr));
+    rr_.check(rbt_download(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
+    rr_.check(rbt_sync(rr_.handle(), nullptr));
+  }
   /// Host wire records of the schedule in force (rbt_stage_layout.h): what an adaptor sends instead of the dense records.
   /// device_inverse_dynamics: the records leave M and the ID rows of dIDCdqv / IDC to the device (RBT_WIRE_DEVICE_ID).
-  void setWireCostStructure(bool robotoc_costs, bool device_inverse_dynamics = false) {
-    cost_structure_ = (robotoc_costs ? RBT_COST_ROBOTOC : RBT_COST_GENERAL) | (device_inverse_dynamics ? RBT_WIRE_DEVICE_ID : 0);
+  /// device_contact_kinematics: the records leave J and the contact rows of dIDCdqv / IDC to the device (RBT_WIRE_DEVICE_CONTACT).
+  void setWireCostStructure(bool robotoc_costs, bool device_inverse_dynamics = false, bool device_contact_kinematics = false) {
+    cost_structure_ = (robotoc_costs ? RBT_COST_ROBOTOC : RBT_COST_GENERAL) | (device_inverse_dynamics ? RBT_WIRE_DEVICE_ID : 0) |
+                      (device_contact_kinematics ? RBT_WIRE_DEVICE_CONTACT : 0);
     rr_.check(rbt_set_wire_cost_structure(rr_.handle(), cost_structure_));
   }
   std::vector<double> packWire(const std::vector<double>& lin, const std::vector<rbt_stage_ctrl>& ctrl) const {

@@ -24,6 +24,7 @@
 #include "eval_kernels.cuh"
 #include "line_search_kernels.cuh"
 #include "rnea_kernels.cuh"
+#include "contact_kernels.cuh"
 
 namespace {
 
@@ -113,7 +114,7 @@ struct Copy {
   bool up;
   int host;
 };
-enum { IN_KKT, IN_WIRE, IN_LIN, IN_CON, IN_SOL, IN_RES, IN_DX0, N_IN };
+enum { IN_KKT, IN_WIRE, IN_LIN, IN_CON, IN_SOL, IN_RES, IN_DX0, IN_CPOS, N_IN };
 enum { OUT_SOL, OUT_CON, OUT_STEPS, N_OUT };
 
 // What an RBT_BUF_* id names on a handle.
@@ -178,6 +179,9 @@ struct rbt_handle {
   DevBuf<int> d_tgt;                  // box rows per PDIPM target (stage_kernels.cuh: StageParams::tgt)
   DevBuf<double> d_limits;            // joint limits per box row (rbt_set_joint_limits)
   DevBuf<rbt::RneaModel> d_model;     // robot model of rbt_linearize_inverse_dynamics (rbt_set_robot_model)
+  DevBuf<double> d_gains;             // Baumgarte gains per contact (rbt_set_contact_gains)
+  DevBuf<double> d_cpos;              // desired contact positions (RBT_BUF_CONTACT_POS), allocated on the first upload
+  bool cpos_set = false;              // d_cpos has been uploaded once
   // line search (line_search_kernels.cuh): trial buffers sized on first use, filter state per OCP
   int ls_trials = 0;
   DevBuf<double> d_ls_alphas, d_ls_trial, d_ls_stage_barrier, d_ls_barrier, d_ls_in, d_ls_filt, d_ls_step;
@@ -354,6 +358,7 @@ static BufDesc buf(rbt_handle* h, int which) {
       /* XDIR  */ {h->d_xd.get(), S.x_stride, SC_GRID, true, &h->d_xd, -1},
       /* STEPS */ {h->d_steps.get(), 2, SC_OCP, true, nullptr, -1},
       /* PERF  */ {h->d_perf.get(), 8, SC_OCP, true, nullptr, -1},
+      /* CPOS  */ {h->d_cpos.get(), 3 * S.ncon, SC_GRID, true, nullptr, IN_CPOS},
   };
   return which >= 0 && which < int(sizeof(t) / sizeof(t[0])) ? t[which] : BufDesc{nullptr, 0, SC_NONE, false, nullptr, -1};
 }
@@ -467,6 +472,10 @@ static std::vector<Copy> iteration_plan(const rbt_handle* h, int mode, long long
 // The copies of rbt_upload into buffer `in` (IN_*), over the whole batch.
 static std::vector<Copy> upload_plan(const rbt_handle* h, int in) {
   if (in == IN_KKT) return kkt_plan(h);
+  if (in == IN_CPOS) {  // contiguous [batch][n_grid][n_contacts][3]
+    const size_t n = size_t(h->batch) * h->n_grid * 3 * h->S.ncon;
+    return {{h->d_cpos.get(), 0, n, n, 1, true, IN_CPOS}};
+  }
   std::vector<Copy> v;
   for (const Copy& c : iteration_plan(h, MODE_DENSE, 0, full(h)))
     if (c.up && c.host == in) v.push_back(c);
@@ -514,6 +523,10 @@ int rbt_upload(rbt_handle* h, int which, const double* host, void* stream) {
   if (h->n_grid == 0) return RBT_ERR_STATE;
   RBT_CUDA(h, cudaSetDevice(h->device));
   if (which == RBT_BUF_KKT) h->kkt_from_condense = false;
+  if (which == RBT_BUF_CONTACT_POS) {
+    RBT_CUDA(h, h->d_cpos.ensure(size_t(h->batch) * h->n_grid_max * 3 * h->S.ncon));
+    h->cpos_set = true;
+  }
   const double* in[N_IN] = {};
   in[d.in] = host;
   return issue(h, upload_plan(h, d.in), true, in, nullptr, (cudaStream_t)stream, "rbt_upload");
@@ -522,6 +535,10 @@ int rbt_upload(rbt_handle* h, int which, const double* host, void* stream) {
 int rbt_download(rbt_handle* h, int which, double* host, void* stream) {
   if (!h || !host) return RBT_ERR_ARG;
   const BufDesc d = buf(h, which);
+  if (which == RBT_BUF_CONTACT_POS && h->stage_ready && !d.ptr) {
+    h->err = "[rbt_download] RBT_BUF_CONTACT_POS has not been uploaded yet";
+    return RBT_ERR_STATE;
+  }
   if (!d.ptr) return RBT_ERR_ARG;
   if (h->n_grid == 0) return RBT_ERR_STATE;
   RBT_CUDA(h, cudaSetDevice(h->device));
@@ -1123,6 +1140,49 @@ int rbt_linearize_inverse_dynamics(rbt_handle* h, void* stream) {
   return inverse_dynamics(h, full(h), (cudaStream_t)stream);
 }
 
+int rbt_set_contact_gains(rbt_handle* h, const double* gains_host) {
+  if (!h || !gains_host) return RBT_ERR_ARG;
+  if (!h->stage_ready) {
+    h->err = "[rbt_set_contact_gains] stage layer not set up";
+    return RBT_ERR_STATE;
+  }
+  for (int e = 0; e < 2 * h->S.ncon; ++e)
+    if (!(gains_host[e] >= 0.0 && gains_host[e] < HUGE_VAL)) {
+      h->err = "[rbt_set_contact_gains] invalid argument: contact " + std::to_string(e / 2) +
+               (e % 2 ? ": velocity" : ": position") + " gain must be finite and non-negative";
+      return RBT_ERR_ARG;
+    }
+  RBT_CUDA(h, cudaSetDevice(h->device));
+  RBT_CUDA(h, h->d_gains.ensure(2 * RBT_MAX_CONTACTS));
+  RBT_CUDA(h, cudaMemcpy(h->d_gains.get(), gains_host, sizeof(double) * 2 * h->S.ncon, cudaMemcpyHostToDevice));
+  return RBT_OK;
+}
+
+// what rbt_linearize_contact_kinematics needs besides the stage layer: the model, the gains and the desired positions
+static const char* contact_kinematics_missing(const rbt_handle* h) {
+  if (!h->d_model.get()) return "call rbt_set_robot_model first";
+  if (!h->d_gains.get()) return "call rbt_set_contact_gains first";
+  if (!h->cpos_set) return "upload RBT_BUF_CONTACT_POS first";
+  return nullptr;
+}
+
+static int contact_kinematics(rbt_handle* h, Win w, cudaStream_t st) {
+  rbt::linearize_contact_kinematics_kernel<CNV><<<w.nb * h->n_grid, rbt::ContactCfg<CNV>::NTHR, 0, st>>>(
+      make_stage_params(h, w), h->d_model.get(), h->d_gains.get(), h->d_cpos.get() + w.rec() * 3 * h->S.ncon);
+  RBT_CUDA(h, cudaGetLastError());
+  h->launches += 1;
+  return RBT_OK;
+}
+
+int rbt_linearize_contact_kinematics(rbt_handle* h, void* stream) {
+  RBT_STAGE_CHECK(h, "rbt_linearize_contact_kinematics");
+  if (const char* why = contact_kinematics_missing(h)) {
+    h->err = std::string("[rbt_linearize_contact_kinematics] ") + why;
+    return RBT_ERR_STATE;
+  }
+  return contact_kinematics(h, full(h), (cudaStream_t)stream);
+}
+
 int rbt_initial_state_direction(rbt_handle* h, const double* dq0_v0_host, void* stream) {
   RBT_STAGE_CHECK(h, "rbt_initial_state_direction");
   if (!dq0_v0_host) return RBT_ERR_ARG;
@@ -1259,6 +1319,12 @@ static int iteration_host_impl(rbt_handle* h, const double* wire_host, const dou
       h->err = "[rbt_iteration_host_wire] the wire records leave the inverse dynamics to the device: call rbt_set_robot_model first";
       return RBT_ERR_STATE;
     }
+    if (h->cost_structure & RBT_WIRE_DEVICE_CONTACT) {
+      if (const char* why = contact_kinematics_missing(h)) {
+        h->err = std::string("[rbt_iteration_host_wire] the wire records leave the contact rows to the device: ") + why;
+        return RBT_ERR_STATE;
+      }
+    }
     if (sw && !lin_host) {
       h->err = "[rbt_iteration_host_wire] invalid argument: the schedule has switching-constraint stages, their sections come from lin_host_switching";
       return RBT_ERR_ARG;
@@ -1320,6 +1386,7 @@ static int iteration_host_impl(rbt_handle* h, const double* wire_host, const dou
       rbt::unpack_wire_kernel<<<w.nb * h->n_grid, 128, 0, st>>>(wp);
       h->launches += 1;
       if ((h->cost_structure & RBT_WIRE_DEVICE_ID) && (rc = inverse_dynamics(h, w, st))) return rc;
+      if ((h->cost_structure & RBT_WIRE_DEVICE_CONTACT) && (rc = contact_kinematics(h, w, st))) return rc;
     }
     if ((rc = condense(h, w, st)) || (rc = backward(h, 0, w, st)) || (rc = forward(h, w, st)) || (rc = expand(h, w, st)) ||
         (rc = update(h, w, st)))
@@ -1359,7 +1426,7 @@ int rbt_iteration_host_resident(rbt_handle* h, const double* wire_host, const do
 }
 
 int rbt_set_wire_cost_structure(rbt_handle* h, int cost_structure) {
-  if (!h || (cost_structure & ~(RBT_COST_ROBOTOC | RBT_WIRE_DEVICE_ID)) != 0) return RBT_ERR_ARG;
+  if (!h || (cost_structure & ~(RBT_COST_ROBOTOC | RBT_WIRE_DEVICE_ID | RBT_WIRE_DEVICE_CONTACT)) != 0) return RBT_ERR_ARG;
   if (h->cost_structure != cost_structure) h->wire_dirty = true;
   h->cost_structure = cost_structure;
   return RBT_OK;

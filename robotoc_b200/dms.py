@@ -16,9 +16,10 @@ import numpy as np
 from .riccati import RiccatiRecursion, _check, _vp
 from .stage import StageDims, StageLayout
 
-LIN, CON, EXP, SOL, XDIR, STEPS, PERF = 6, 7, 8, 9, 10, 11, 12
+LIN, CON, EXP, SOL, XDIR, STEPS, PERF, CONTACT_POS = 6, 7, 8, 9, 10, 11, 12, 13
 RBT_MAX_BODIES, RBT_MAX_CONTACTS = 32, 8
 WIRE_DEVICE_ID = 2  # RBT_WIRE_DEVICE_ID (rbt_stage_layout.h)
+WIRE_DEVICE_CONTACT = 4  # RBT_WIRE_DEVICE_CONTACT
 
 
 class rbt_robot_model(ctypes.Structure):
@@ -95,6 +96,30 @@ class DirectMultipleShooting:
         solution records."""
         _check(self._lib.rbt_linearize_inverse_dynamics(self._h, stream), self.rr._err, "DirectMultipleShooting")
 
+    def setContactGains(self, gains):
+        """Baumgarte gains [n_contacts, 2] = {position gain, velocity gain} of each point contact (ContactModelInfo), for
+        linearizeContactKinematics and the device-side contact rows of the wire paths."""
+        gains = np.ascontiguousarray(gains, dtype=np.float64)
+        if gains.shape != (self.sdims.n_contacts, 2):
+            raise ValueError(f"[DirectMultipleShooting] invalid argument: gains must have shape {(self.sdims.n_contacts, 2)}")
+        _check(self._lib.rbt_set_contact_gains(self._h, _vp(gains)), self.rr._err, "DirectMultipleShooting")
+
+    def setContactPositions(self, pos, stream=None):
+        """Desired contact positions [batch, n_grid, n_contacts, 3] (ContactStatus::contactPosition of each grid point's phase),
+        read for the active contacts of Intermediate / Lift grid points.  Resident: upload again when the planner changes them."""
+        pos = np.ascontiguousarray(pos, dtype=np.float64)
+        shape = (self.rr.batch, self.rr.n_grid, self.sdims.n_contacts, 3)
+        if pos.shape != shape:
+            raise ValueError(f"[DirectMultipleShooting] invalid argument: contact positions must have shape {shape}")
+        _check(self._lib.rbt_upload(self._h, CONTACT_POS, _vp(pos), stream), self.rr._err, "DirectMultipleShooting")
+        self.rr.synchronize(stream)
+
+    def linearizeContactKinematics(self, stream=None):
+        """The contact rows of linearizeContactDynamics / linearizeImpactDynamics on the device
+        (rbt_linearize_contact_kinematics): J, the contact rows of dIDCdqv and IDC, and the multiplier terms of lf, lq, lv,
+        la | ldv, from the resident solution records (setRobotModel, setContactGains and setContactPositions first)."""
+        _check(self._lib.rbt_linearize_contact_kinematics(self._h, stream), self.rr._err, "DirectMultipleShooting")
+
     def computeStepSizes(self, stream=None):
         _check(self._lib.rbt_expand_and_step_sizes(self._h, stream), self.rr._err, "DirectMultipleShooting")
 
@@ -167,12 +192,17 @@ class DirectMultipleShooting:
                self.rr._err, "DirectMultipleShooting")
         return h2d.value, d2h.value
 
-    def setWireCostStructure(self, robotoc_costs: bool, device_inverse_dynamics: bool = False):
+    def setWireCostStructure(self, robotoc_costs: bool, device_inverse_dynamics: bool = False,
+                             device_contact_kinematics: bool = False):
         """Which cost-Hessian structure the host's wire records have: False = general (full packed triangles of Qxx, Quu, Qff),
         True = what robotoc's shipped cost components produce (Qqq dense, Qvv / Quu / Qff diagonal, Qqv = 0).
         device_inverse_dynamics: the wire records leave out M and the ID rows of dIDCdqv and IDC (and their gradients the beta
-        terms); iteration_host_wire / iteration_host_resident compute them on the device (setRobotModel first)."""
-        self._cost_structure = (1 if robotoc_costs else 0) | (WIRE_DEVICE_ID if device_inverse_dynamics else 0)
+        terms); iteration_host_wire / iteration_host_resident compute them on the device (setRobotModel first).
+        device_contact_kinematics: the wire records leave out J and the contact rows of dIDCdqv and IDC (and their gradients
+        the multiplier terms of those rows); the wire paths compute them on the device (setRobotModel, setContactGains and
+        setContactPositions first)."""
+        self._cost_structure = ((1 if robotoc_costs else 0) | (WIRE_DEVICE_ID if device_inverse_dynamics else 0)
+                                | (WIRE_DEVICE_CONTACT if device_contact_kinematics else 0))
         _check(self._lib.rbt_set_wire_cost_structure(self._h, self._cost_structure), self.rr._err, "DirectMultipleShooting")
 
     def pack_wire(self, lin):

@@ -1,0 +1,60 @@
+"""Builds and runs tests/cpp/test_contact_kinematics.cpp: the C++ adaptor's setContactGains / setContactPositions /
+linearizeContactKinematics and the resident wire path with the inverse dynamics and the contact rows left to the device.  The
+records the C++ side writes are checked here against the numpy restatement tests/contact_ref.py."""
+import ctypes
+import os
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+sys.path.insert(0, os.path.join(HERE, "golden"))
+import contact_ref as CR  # noqa: E402
+import make_model_fixture  # noqa: E402
+import rbd_ref as R  # noqa: E402
+from helpers import rel_err  # noqa: E402
+
+
+def _build(tmp):
+    exe = os.path.join(tmp, "test_contact_kinematics")
+    gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
+    cmd = [gxx, "-std=c++14", "-O1", "-I", os.path.join(ROOT, "include"), os.path.join(HERE, "cpp", "test_contact_kinematics.cpp"),
+           "-L", os.path.join(ROOT, "robotoc_b200"), "-lrobotoc_b200", "-Wl,-rpath," + os.path.join(ROOT, "robotoc_b200"), "-o", exe]
+    subprocess.run(cmd, check=True)
+    return exe
+
+
+def test_cpp_contact_kinematics_test_compiles_and_links(tmp_path):
+    """CPU: the adaptor's new methods compile as C++14 and link against the C ABI."""
+    assert os.path.exists(_build(str(tmp_path)))
+
+
+@pytest.mark.gpu
+# random2: a seeded tree whose four contacts have a full-rank stacked Jacobian, so the iteration's J M^-1 J^T is positive definite
+# (random1's four contacts span only 11 of 12 rows)
+@pytest.mark.parametrize("model", ["anymal", "random2"])
+def test_cpp_contact_kinematics(tmp_path, model):
+    from robotoc_b200 import ANYMAL, StageDims, StageLayout, anymal_constraint_table
+    from robotoc_b200._lib import rbt_stage_ctrl
+    exe = _build(str(tmp_path))
+    m = make_model_fixture.load() if model == "anymal" else R.random_model(int(model[-1]))
+    mpath = os.path.join(str(tmp_path), "model.bin")
+    with open(mpath, "wb") as f:
+        f.write(bytes(R.to_c(m)))
+    out = subprocess.run([exe, mpath, str(tmp_path)], capture_output=True, text=True, timeout=120)
+    print(out.stdout, out.stderr)
+    assert out.returncode == 0, out.stdout + out.stderr
+    table = anymal_constraint_table()
+    S = StageLayout(StageDims(ANYMAL, nf_max=12, n_contacts=4, n_box=table.n_box))
+    raw = open(os.path.join(str(tmp_path), "ctrl.bin"), "rb").read()
+    n_grid = len(raw) // ctypes.sizeof(rbt_stage_ctrl)
+    ctrl = (rbt_stage_ctrl * n_grid).from_buffer_copy(raw)
+    load = lambda name, stride: np.fromfile(os.path.join(str(tmp_path), name)).reshape(-1, n_grid, stride)  # noqa: E731
+    sol, lin_in, lin_out = load("sol.bin", S.s_stride), load("lin_in.bin", S.l_stride), load("lin_out.bin", S.l_stride)
+    gains = np.fromfile(os.path.join(str(tmp_path), "gains.bin")).reshape(4, 2)
+    pos = np.fromfile(os.path.join(str(tmp_path), "pos.bin")).reshape(-1, n_grid, 4, 3)
+    ref = CR.linearize(m, S, ctrl, sol, lin_in, gains, pos)
+    assert rel_err(lin_out, ref) < 1e-12
