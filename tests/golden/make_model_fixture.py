@@ -1,11 +1,14 @@
 """Writes tests/golden/anymal_model.npz: the robot model (fields of rbt_robot_model) of the reference's ANYmal example, parsed
 from examples/anymal/anymal_b_simple_description/urdf/anymal.urdf with the standard-library XML parser the way Pinocchio's URDF
 parser builds a pinocchio::Model with a JointModelFreeFlyer root:
-  - joints in depth-first order of the kinematic tree (children in file order), the root link on the free flyer;
+  - joints in depth-first order of the kinematic tree, the root link on the free flyer; each link's child joints are visited in
+    the order of their names, because urdfdom builds a link's child list by walking its std::map of joints keyed by name (this
+    gives the legs LF, LH, RF, RH, the order the reference's examples write q in);
   - a fixed joint merges its child link into the parent body: the link's inertia is added in the body's joint frame, and its frame
     (e.g. LF_FOOT) is placed in the parent joint's frame;
   - a revolute joint's placement = (fixed-joint chain from its parent body to its parent link) * its URDF origin;
   - contacts LF_FOOT, LH_FOOT, RF_FOOT, RH_FOOT (examples/anymal/trot.cpp:34-37), gravity (0, 0, -9.81).
+The npz also holds the revolute joint names in q order ("joint_names") and the contact frame names ("contact_names").
 Runs only where a reference tree exists: ROBOTOC_REFERENCE=/path/to/robotoc python tests/golden/make_model_fixture.py"""
 import os
 import sys
@@ -70,10 +73,10 @@ def parse(urdf):
     links = {l.get("name"): l for l in root.findall("link")}
     joints = root.findall("joint")
     children = {}
-    for j in joints:
+    for j in sorted(joints, key=lambda j: j.get("name")):
         children.setdefault(j.find("parent").get("link"), []).append(j)
     root_link = (set(links) - {j.find("child").get("link") for j in joints}).pop()
-    parent, axis, placement, inertias, frames = [-1], [np.zeros(3)], [(np.eye(3), np.zeros(3))], [], {}
+    parent, axis, placement, inertias, frames, names = [-1], [np.zeros(3)], [(np.eye(3), np.zeros(3))], [], {}, []
     inertias.append((0.0, np.zeros(3), np.zeros((3, 3))))
 
     def visit(link, body, T):
@@ -89,6 +92,7 @@ def parse(urdf):
                 ax = j.find("axis")
                 u = np.array([float(x) for x in (ax.get("xyz") if ax is not None else "1 0 0").split()])
                 parent.append(body)
+                names.append(j.get("name"))
                 axis.append(u / np.linalg.norm(u))
                 placement.append(compose(T, O))
                 inertias.append((0.0, np.zeros(3), np.zeros((3, 3))))
@@ -107,6 +111,7 @@ def parse(urdf):
         "contact_parent": np.array([frames[c][0] for c in CONTACTS]),
         "contact_placement": np.array([pack(frames[c][1]) for c in CONTACTS]),
         "gravity": np.array([0.0, 0.0, -9.81]),
+        "joint_names": np.array(names), "contact_names": np.array(CONTACTS),
     }
 
 
