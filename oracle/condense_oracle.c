@@ -13,7 +13,10 @@
  * updated slack / dual) on event schedules with and without STO and on the BASELINE trot N=40 schedule: agreement < 1e-10
  * (measured 1e-14), and against the committed reference output tests/golden/golden_ref_stage_r2.npz.  Not covered by the
  * reference code here: Robot::computeMJtJinv (Pinocchio; dense restatement on both sides) and SplitSolution::integrate's SE(3)
- * exponential (Pinocchio; pinned against scipy's Rotation in tests/test_oracle_condense.py).
+ * exponential (Pinocchio; pinned against scipy's Rotation in tests/test_oracle_condense.py, and against a 100-digit expm in
+ * tests/test_stage_mp.py).  The exponential here takes 1 - cos th as 2 sin^2(th/2), as the CUDA kernel does, where pinocchio's
+ * exp6 writes (1 - cos th) / th^2: the same function, without the cancellation that costs the difference form up to 2u / th^2
+ * of it just above the small-angle branch.  This is a choice of accuracy, not a departure from the reference's mathematics.
  * Additionally pinned by identities that do not reuse its formulas (tests/test_oracle_condense.py): MJtJinv == dense inverse;
  * condensed quadratic model == uncondensed model with (a, f) substituted; PDIPM condensing == J^T diag(z/s) J; the expansions
  * satisfy the linearised contact dynamics / make the uncondensed stage Lagrangian stationary; STO sensitivities == substituted
@@ -527,7 +530,9 @@ static void integrate_free_flyer(double* q, const double* dq, double step) {
   if (th < 1e-6) {
     b = 0.5 - th2 / 24.0; cc = 1.0 / 6.0 - th2 / 120.0;
   } else {
-    b = (1.0 - cos(th)) / th2; cc = (th - sin(th)) / (th2 * th);
+    /* 1 - cos th = 2 sin^2(th/2): the difference form loses up to 2u / th^2 of b (9e-5 relative just above th = 1e-6) */
+    const double s2 = sin(0.5 * th), c2 = cos(0.5 * th);
+    b = 2.0 * s2 * s2 / th2; cc = (th - 2.0 * s2 * c2) / (th2 * th);
   }
   /* t = V v,  V = I + b [w]x + cc [w]x^2 */
   const double cx = wy * vz - wz * vy, cy = wz * vx - wx * vz, cz = wx * vy - wy * vx;
