@@ -66,15 +66,52 @@ def _kkt_lin(sd, S, ctrl, pad):
     return np.ascontiguousarray(lin), np.ascontiguousarray(con)
 
 
-def _condense(pad):
+def _unread_pdipm(S, table, ctrl, lin, con, pad):
+    """Fills what robotoc does not read of the PDIPM inputs with `pad`: the slack, dual and residual of gated box rows (grid
+    points 0 and 1, Impact grid points) and of inactive contacts' cone rows, and those contacts' dg/dq | dg/df.  Returns the
+    number of entries filled."""
+    import condense_mp
+    from make_condense_mp import row_levels
+    n = 0
+    for i, c in enumerate(ctrl):
+        if c.type == condense_mp.TERMINAL:
+            continue
+        g = condense_mp.unpack(S, table, c, row_levels(table), lin[0, i], con[0, i])
+        for r in sorted(set(range(S.nc)) - set(condense_mp.acting_rows(g)[0])):
+            for f in (S.c_slack, S.c_dual, S.c_res):
+                con[:, i, f + r] = pad
+                n += con.shape[0]
+        for ci in range(S.ncon):
+            if not (c.contact_mask >> ci) & 1:
+                lin[:, i, S.l_dgdq + ci * 5 * S.nv:S.l_dgdq + (ci + 1) * 5 * S.nv] = pad
+                lin[:, i, S.l_dgdf + ci * 15:S.l_dgdf + (ci + 1) * 15] = pad
+                n += con.shape[0] * (5 * S.nv + 15)
+    return n
+
+
+def _condense(pad, unread=None):
+    """Condensing of the K1 cases; with `unread`, also the expansion (of a fixed direction) on inputs whose unread PDIPM
+    entries hold `unread` (_unread_pdipm)."""
+    from robotoc_b200 import anymal_constraint_table
     ctrl = _kkt_schedule()
     rr, dms, sd, S, K = _setup(ctrl, len(G.STATES))
     try:
         lin, con = _kkt_lin(sd, S, ctrl, pad)
+        if unread is not None:
+            _unread_pdipm(S, anymal_constraint_table(), ctrl, lin, con, unread)
         dms.condense(lin, con)
         out = {"lin": dms._down(LIN, lin.shape), "ex": dms.getExpansionData(), "kkt": dms.getKKT(),
                "con": dms.getConstraintData()}
         assert int(rr.info().max()) == 0
+        if unread is not None:
+            import torch
+            d = np.random.default_rng(5).uniform(-1, 1, (len(G.STATES), len(ctrl), K.d_stride))
+            dir_t = torch.from_numpy(d).cuda()
+            rr.bind_buffer(DIR, ctypes.c_void_p(dir_t.data_ptr()))
+            torch.cuda.synchronize()
+            dms.computeStepSizes()
+            out.update(con_exp=dms.getConstraintData(), xd=dms.getExpandedDirection(),
+                       steps=np.stack([dms.maxPrimalStepSize(), dms.maxDualStepSize()], 1))
     finally:
         rr.close()
     return ctrl, S, out
@@ -98,14 +135,21 @@ def test_mjtjinv_matches_the_extended_precision_reference():
 
 
 def test_condensing_reads_no_inactive_contact_row_of_j():
-    """NaN in the rows of J beyond nf (the kernels' contract: only the active contact rows are read) gives, bit for bit, the
-    expansion, KKT and PDIPM records of zeros there."""
-    _, S, zero = _condense(0.0)
-    ctrl, _, nan = _condense(np.nan)
+    """NaN in every input robotoc does not read -- the rows of J beyond nf, the slack, dual and residual of gated box rows
+    and of inactive contacts' cone rows, and those contacts' cone Jacobians -- gives, bit for bit, the expansion, KKT and
+    PDIPM records, the expanded direction and the step sizes of the inputs with zeros (J) and finite values (PDIPM) there.
+    The slack, dual and residual fields themselves are inputs, so the PDIPM records are compared from cmpl on; robotoc
+    writes dslack = ddual = 1 on inactive cone rows (friction_cone.cpp:244-245), on both runs."""
+    _, S, zero = _condense(0.0, unread=0.5)
+    ctrl, _, nan = _condense(np.nan, unread=np.nan)
     poisoned = sum(int(np.isnan(nan["lin"][:, i, S.l_J:S.l_J + 216]).sum()) for i in range(len(ctrl) - 1))
     assert poisoned == len(G.STATES) * sum((12 - G.nf_of(int(m))) * 18 * len(TYPES) for m in G.MASKS), "the NaNs did not land"
-    for key in ("ex", "kkt", "con"):
+    assert np.isnan(nan["lin"][:, :, S.l_dgdq:S.l_dgdq + 5 * S.nv]).any()
+    for key in ("ex", "kkt", "xd", "steps"):
         np.testing.assert_array_equal(nan[key].view(np.uint64), zero[key].view(np.uint64), err_msg=key)
+    for key in ("con", "con_exp"):
+        np.testing.assert_array_equal(nan[key][..., S.c_cmpl:].view(np.uint64), zero[key][..., S.c_cmpl:].view(np.uint64),
+                                      err_msg=key)
 
 
 class _DeviceView:
