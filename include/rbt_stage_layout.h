@@ -192,6 +192,11 @@ enum { RBT_COST_GENERAL = 0, RBT_COST_ROBOTOC = 1 };
 /* OR-ed into cost_structure: the device fills the contact rows (rbt_linearize_contact_kinematics), so non-terminal wire records
  * carry neither J nor the nf contact rows of dIDCdqv and IDC; alone or together with RBT_WIRE_DEVICE_ID */
 #define RBT_WIRE_DEVICE_CONTACT 4
+/* OR-ed into cost_structure: the device fills the state-equation rows (rbt_linearize_state_equation), so non-terminal wire
+ * records carry neither Fx nor the three SE(3) blocks (the lx .. SE(3) segment splits around them) and terminal records no
+ * Fqq_prev block; the STO section still travels with the cost's share of h, hv, ha (the device adds the costate terms and
+ * overwrites fx).  Alone or together with the other two bits */
+#define RBT_WIRE_DEVICE_STATE 16
 #define RBT_WIRE_MAX_SEGS 20
 #define RBT_WIRE_MAX_ZERO 5
 typedef struct rbt_wire_layout {
@@ -225,13 +230,14 @@ static inline RBT_HD void rbt_make_wire_layout(const rbt_stage_layout* L, const 
   const int nv = L->nv, nx = L->nx, nf = c->nf, nvf = nv + nf;
   const int dc = ((cost_structure & RBT_COST_ROBOTOC) != 0), did = ((cost_structure & RBT_WIRE_DEVICE_ID) != 0);
   const int dcon = ((cost_structure & RBT_WIRE_DEVICE_CONTACT) != 0);
+  const int dst = ((cost_structure & RBT_WIRE_DEVICE_STATE) != 0);
   int ci;
   cost_structure &= RBT_COST_ROBOTOC;
   W->nseg = 0; W->nzero = 0; W->w_doubles = 0; W->ocp_off = 0;
   if (c->type == RBT_TERMINAL) {
     rbt_wire_add_qxx_(L, cost_structure, W);
     rbt_wire_add_(W, L->l_lx, nx, 1, nx, 0);
-    rbt_wire_add_(W, L->l_se3 + 36, 36, 1, 36, 0);
+    if (!dst) rbt_wire_add_(W, L->l_se3 + 36, 36, 1, 36, 0);
     return;
   }
   if (!did && dcon) {  /* ID rows only: M, [dIDdq | dIDdv], ID */
@@ -254,7 +260,12 @@ static inline RBT_HD void rbt_make_wire_layout(const rbt_stage_layout* L, const 
   rbt_wire_add_qxx_(L, cost_structure, W);
   if (dc) rbt_wire_zero_(W, L->l_Quu, L->nu * L->nu);
   rbt_wire_add_(W, L->l_Quu, L->nu, L->nu, L->nu, dc ? 2 : 1);
-  rbt_wire_add_(W, L->l_lx, L->l_Phix - L->l_lx, 1, L->l_Phix - L->l_lx, 0);   /* lx | la | lf | lu | Fx | lup | SE(3) blocks */
+  if (dst) {  /* lx | la | lf | lu, then lup */
+    rbt_wire_add_(W, L->l_lx, L->l_Fx - L->l_lx, 1, L->l_Fx - L->l_lx, 0);
+    rbt_wire_add_(W, L->l_lup, L->l_se3 - L->l_lup, 1, L->l_se3 - L->l_lup, 0);
+  } else {
+    rbt_wire_add_(W, L->l_lx, L->l_Phix - L->l_lx, 1, L->l_Phix - L->l_lx, 0);   /* lx | la | lf | lu | Fx | lup | SE(3) blocks */
+  }
   for (ci = 0; ci < L->ncon; ++ci)
     if ((c->contact_mask >> ci) & 1) {
       rbt_wire_add_(W, L->l_dgdq + ci * 5 * nv, 5 * nv, 1, 5 * nv, 0);

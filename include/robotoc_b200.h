@@ -51,8 +51,10 @@ enum {
   RBT_BUF_STEPS = 11,/* [batch][2] max primal / dual step size over the horizon */
   RBT_BUF_PERF = 12, /* [batch][8] PerformanceIndex of rbt_eval_kkt: {cost (0: not evaluated on this path), cost_barrier,
                         primal_feasibility, dual_feasibility, kkt_error, sqrt(kkt_error) = OCPSolver::KKTError(), 0, 0} */
-  RBT_BUF_CONTACT_POS = 13  /* [batch][n_grid][n_contacts][3] desired contact positions of rbt_linearize_contact_kinematics
+  RBT_BUF_CONTACT_POS = 13, /* [batch][n_grid][n_contacts][3] desired contact positions of rbt_linearize_contact_kinematics
                                (ContactStatus::contactPosition of each grid point's phase); allocated by its first upload */
+  RBT_BUF_Q0 = 14           /* [batch][nq] measured configuration q0 of OCPSolver::solve(t, q, v), the q_prev of grid point 0 in
+                               rbt_linearize_state_equation; allocated by its first upload */
 };
 
 typedef struct rbt_handle rbt_handle;
@@ -243,6 +245,19 @@ int rbt_set_contact_gains(rbt_handle* h, const double* gains_host);
  * rbt_linearize_contact_kinematics -> rbt_eval_kkt / rbt_condense.  RBT_ERR_STATE until rbt_set_robot_model,
  * rbt_set_contact_gains and one rbt_upload(RBT_BUF_CONTACT_POS) have been made. */
 int rbt_linearize_contact_kinematics(rbt_handle* h, void* stream);
+/* The state-equation rows (SURVEY.md 8f-1, third slice): linearizeStateEquation (src/dynamics/state_equation.cpp:30-65) on
+ * Intermediate and Lift grid points, linearizeImpactStateEquation (impact_state_equation.cpp:26-54) on Impact grid points and
+ * linearizeTerminalStateEquation (terminal_state_equation.cpp:8-28) on the terminal one, with q_prev = q0 (RBT_BUF_Q0) on grid
+ * point 0 and s[i-1].q otherwise, s_next = s[i+1] (direct_multiple_shooting.cpp:129-159).  Writes Fx = [Fq | Fv], the three
+ * SE(3) blocks at l_se3 (Fqq = dSubtractConfiguration_dqf(q, q_next), Fqq_prev = dSubtractConfiguration_dq0(q_prev, q),
+ * Fqq_cur = dSubtractConfiguration_dq0(q, q_next), state_equation.cpp:78) and, on the terminal grid point, Fqq_prev only; adds
+ * the costate terms to lq, lv and la (impact: ldv); on schedules with a switching-time stage, Intermediate and Lift grid
+ * points also get the STO terms: fx = [v | a] is written, lmd_next . v + gmm_next . a is added to h, lmd_next to hv and
+ * gmm_next to ha.  Every other section is untouched.
+ * Order: rbt_upload(LIN, SOL) -> (rbt_linearize_inverse_dynamics) -> (rbt_linearize_contact_kinematics) ->
+ * rbt_linearize_state_equation -> rbt_eval_kkt / rbt_condense.  RBT_ERR_STATE before rbt_stage_setup or before one
+ * rbt_upload(RBT_BUF_Q0). */
+int rbt_linearize_state_equation(rbt_handle* h, void* stream);
 /* computeInitialStateDirection (src/dynamics/state_equation.cpp:98-109) into RBT_BUF_DX0.  dq0_v0_host: [batch][2 nv] =
  * {q0 (-) s[0].q from Robot::subtractConfiguration (the robot model stays on the host), v0}; uses the stage-0 Fqq_prev_inv that
  * rbt_condense left in RBT_BUF_EXP and s[0].v of RBT_BUF_SOL, so call it after rbt_condense and before rbt_riccati_forward. */
@@ -320,7 +335,11 @@ int rbt_iteration_host_resident(rbt_handle* h, const double* wire_host, const do
  * rbt_iteration_host_bytes counts the smaller records.  RBT_WIRE_DEVICE_CONTACT, alone or with RBT_WIRE_DEVICE_ID: the device
  * computes the contact rows (rbt_linearize_contact_kinematics, after rbt_set_robot_model, rbt_set_contact_gains and an upload of
  * RBT_BUF_CONTACT_POS), so the records drop J and the contact rows of dIDCdqv and IDC and their gradients lack the multiplier
- * terms of the contact rows; the kernel runs right after the inverse-dynamics kernel (or the unpack). */
+ * terms of the contact rows; the kernel runs right after the inverse-dynamics kernel (or the unpack).  RBT_WIRE_DEVICE_STATE,
+ * alone or with the other two: the device computes the state-equation rows (rbt_linearize_state_equation, after an upload of
+ * RBT_BUF_Q0), so non-terminal records drop Fx and the three SE(3) blocks (144 doubles for nv = 18) and terminal records the
+ * Fqq_prev block (36), and the gradients and the STO section lack the costate terms; the kernel runs last, after the
+ * inverse-dynamics and the contact kernels (ID -> contact -> state, the order the gradient additions keep). */
 int rbt_set_wire_cost_structure(rbt_handle* h, int cost_structure);
 int rbt_wire_doubles(const rbt_stage_dims* sdims, const rbt_stage_ctrl* ctrl, int n_grid, int cost_structure);   /* doubles per OCP */
 int rbt_wire_layout_get(const rbt_stage_dims* sdims, const rbt_stage_ctrl* ctrl, int n_grid, int cost_structure, int i,

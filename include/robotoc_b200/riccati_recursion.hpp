@@ -452,12 +452,34 @@ class DirectMultipleShooting {
     rr_.check(rbt_download(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
     rr_.check(rbt_sync(rr_.handle(), nullptr));
   }
+  /// The measured configuration q0 [batch][nq] of OCPSolver::solve(t, q, v), uploaded to RBT_BUF_Q0: grid point 0's q_prev in
+  /// linearizeStateEquation and the device-side state-equation rows of the wire paths.  It stays on the device until the next call.
+  void setInitialConfiguration(const std::vector<double>& q0) {
+    if (q0.size() != size_t(rr_.batch()) * S_.nq)
+      throw std::invalid_argument("[DirectMultipleShooting] invalid argument: q0 must be [batch][nq]");
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_Q0, q0.data(), nullptr));
+    rr_.check(rbt_sync(rr_.handle(), nullptr));
+  }
+  /// The state-equation rows of linearizeStateEquation / linearizeImpactStateEquation / linearizeTerminalStateEquation on the
+  /// device (rbt_linearize_state_equation): `lin` and `sol` are uploaded, `lin` is read back with Fx, the SE(3) blocks, the
+  /// costate terms of the gradients and, on schedules with a switching-time stage, the STO terms filled in.
+  void linearizeStateEquation(std::vector<double>& lin, const std::vector<double>& sol) {
+    expect(lin, S_.l_stride, "lin");
+    expect(sol, S_.s_stride, "sol");
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
+    rr_.check(rbt_upload(rr_.handle(), RBT_BUF_SOL, sol.data(), nullptr));
+    rr_.check(rbt_linearize_state_equation(rr_.handle(), nullptr));
+    rr_.check(rbt_download(rr_.handle(), RBT_BUF_LIN, lin.data(), nullptr));
+    rr_.check(rbt_sync(rr_.handle(), nullptr));
+  }
   /// Host wire records of the schedule in force (rbt_stage_layout.h): what an adaptor sends instead of the dense records.
   /// device_inverse_dynamics: the records leave M and the ID rows of dIDCdqv / IDC to the device (RBT_WIRE_DEVICE_ID).
   /// device_contact_kinematics: the records leave J and the contact rows of dIDCdqv / IDC to the device (RBT_WIRE_DEVICE_CONTACT).
-  void setWireCostStructure(bool robotoc_costs, bool device_inverse_dynamics = false, bool device_contact_kinematics = false) {
+  /// device_state_equation: the records leave Fx and the SE(3) blocks to the device (RBT_WIRE_DEVICE_STATE).
+  void setWireCostStructure(bool robotoc_costs, bool device_inverse_dynamics = false, bool device_contact_kinematics = false,
+                            bool device_state_equation = false) {
     cost_structure_ = (robotoc_costs ? RBT_COST_ROBOTOC : RBT_COST_GENERAL) | (device_inverse_dynamics ? RBT_WIRE_DEVICE_ID : 0) |
-                      (device_contact_kinematics ? RBT_WIRE_DEVICE_CONTACT : 0);
+                      (device_contact_kinematics ? RBT_WIRE_DEVICE_CONTACT : 0) | (device_state_equation ? RBT_WIRE_DEVICE_STATE : 0);
     rr_.check(rbt_set_wire_cost_structure(rr_.handle(), cost_structure_));
   }
   std::vector<double> packWire(const std::vector<double>& lin, const std::vector<rbt_stage_ctrl>& ctrl) const {

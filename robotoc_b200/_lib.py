@@ -27,7 +27,7 @@ EXPORTS = [
     "rbt_create", "rbt_destroy", "rbt_set_schedule", "rbt_dev_ptr", "rbt_buf_doubles", "rbt_bind_buffer", "rbt_upload",
     "rbt_download", "rbt_upload_bytes", "rbt_download_info", "rbt_check_info", "rbt_set_fxx_structure", "rbt_set_time_segments", "rbt_riccati_backward", "rbt_riccati_forward",
     "rbt_riccati_solve_host", "rbt_stage_layout_get", "rbt_stage_setup", "rbt_condense",
-    "rbt_expand_and_step_sizes", "rbt_update", "rbt_trial_doubles", "rbt_line_search_trials", "rbt_line_search_trial_dev", "rbt_line_search_filter", "rbt_line_search_clear_history", "rbt_eval_kkt", "rbt_set_slack_and_dual_positive", "rbt_initial_state_direction", "rbt_set_joint_limits", "rbt_linearize_joint_limits", "rbt_set_robot_model", "rbt_linearize_inverse_dynamics", "rbt_set_contact_gains", "rbt_linearize_contact_kinematics", "rbt_iteration_host", "rbt_iteration_host_bytes", "rbt_iteration_host_wire", "rbt_iteration_host_resident", "rbt_set_wire_cost_structure", "rbt_wire_doubles", "rbt_wire_layout_get", "rbt_pack_wire", "rbt_set_condense_event", "rbt_step_doubles", "rbt_pack_step", "rbt_allgather_step", "rbt_sync", "rbt_last_error", "rbt_launch_count",
+    "rbt_expand_and_step_sizes", "rbt_update", "rbt_trial_doubles", "rbt_line_search_trials", "rbt_line_search_trial_dev", "rbt_line_search_filter", "rbt_line_search_clear_history", "rbt_eval_kkt", "rbt_set_slack_and_dual_positive", "rbt_initial_state_direction", "rbt_set_joint_limits", "rbt_linearize_joint_limits", "rbt_set_robot_model", "rbt_linearize_inverse_dynamics", "rbt_set_contact_gains", "rbt_linearize_contact_kinematics", "rbt_linearize_state_equation", "rbt_iteration_host", "rbt_iteration_host_bytes", "rbt_iteration_host_wire", "rbt_iteration_host_resident", "rbt_set_wire_cost_structure", "rbt_wire_doubles", "rbt_wire_layout_get", "rbt_pack_wire", "rbt_set_condense_event", "rbt_step_doubles", "rbt_pack_step", "rbt_allgather_step", "rbt_sync", "rbt_last_error", "rbt_launch_count",
     "rbt_unconstr_create", "rbt_unconstr_destroy", "rbt_unconstr_dev_ptr", "rbt_unconstr_buf_doubles",
     "rbt_unconstr_upload", "rbt_unconstr_download", "rbt_unconstr_download_info", "rbt_unconstr_backward",
     "rbt_unconstr_forward", "rbt_unconstr_solve_host", "rbt_unconstr_sync", "rbt_unconstr_last_error",
@@ -100,6 +100,7 @@ def lib():
     L.rbt_linearize_inverse_dynamics.argtypes = [c_vp, c_vp]
     L.rbt_set_contact_gains.argtypes = [c_vp, c_vp]
     L.rbt_linearize_contact_kinematics.argtypes = [c_vp, c_vp]
+    L.rbt_linearize_state_equation.argtypes = [c_vp, c_vp]
     L.rbt_set_wire_cost_structure.argtypes = [c_vp, c_int]
     L.rbt_wire_doubles.argtypes = [c_vp, c_vp, c_int, c_int]
     L.rbt_wire_layout_get.argtypes = [c_vp, c_vp, c_int, c_int, c_int, c_vp]

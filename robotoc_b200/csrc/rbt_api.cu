@@ -25,6 +25,7 @@
 #include "line_search_kernels.cuh"
 #include "rnea_kernels.cuh"
 #include "contact_kernels.cuh"
+#include "state_kernels.cuh"
 
 namespace {
 
@@ -114,7 +115,7 @@ struct Copy {
   bool up;
   int host;
 };
-enum { IN_KKT, IN_WIRE, IN_LIN, IN_CON, IN_SOL, IN_RES, IN_DX0, IN_CPOS, N_IN };
+enum { IN_KKT, IN_WIRE, IN_LIN, IN_CON, IN_SOL, IN_RES, IN_DX0, IN_CPOS, IN_Q0, N_IN };
 enum { OUT_SOL, OUT_CON, OUT_STEPS, N_OUT };
 
 // What an RBT_BUF_* id names on a handle.
@@ -182,6 +183,8 @@ struct rbt_handle {
   DevBuf<double> d_gains;             // Baumgarte gains per contact (rbt_set_contact_gains)
   DevBuf<double> d_cpos;              // desired contact positions (RBT_BUF_CONTACT_POS), allocated on the first upload
   bool cpos_set = false;              // d_cpos has been uploaded once
+  DevBuf<double> d_q0;                // measured configuration per OCP (RBT_BUF_Q0), allocated on the first upload
+  bool q0_set = false;                // d_q0 has been uploaded once
   // line search (line_search_kernels.cuh): trial buffers sized on first use, filter state per OCP
   int ls_trials = 0;
   DevBuf<double> d_ls_alphas, d_ls_trial, d_ls_stage_barrier, d_ls_barrier, d_ls_in, d_ls_filt, d_ls_step;
@@ -359,6 +362,7 @@ static BufDesc buf(rbt_handle* h, int which) {
       /* STEPS */ {h->d_steps.get(), 2, SC_OCP, true, nullptr, -1},
       /* PERF  */ {h->d_perf.get(), 8, SC_OCP, true, nullptr, -1},
       /* CPOS  */ {h->d_cpos.get(), 3 * S.ncon, SC_GRID, true, nullptr, IN_CPOS},
+      /* Q0    */ {h->d_q0.get(), S.nq, SC_OCP, true, nullptr, IN_Q0},
   };
   return which >= 0 && which < int(sizeof(t) / sizeof(t[0])) ? t[which] : BufDesc{nullptr, 0, SC_NONE, false, nullptr, -1};
 }
@@ -476,6 +480,10 @@ static std::vector<Copy> upload_plan(const rbt_handle* h, int in) {
     const size_t n = size_t(h->batch) * h->n_grid * 3 * h->S.ncon;
     return {{h->d_cpos.get(), 0, n, n, 1, true, IN_CPOS}};
   }
+  if (in == IN_Q0) {  // contiguous [batch][nq]
+    const size_t n = size_t(h->batch) * h->S.nq;
+    return {{h->d_q0.get(), 0, n, n, 1, true, IN_Q0}};
+  }
   std::vector<Copy> v;
   for (const Copy& c : iteration_plan(h, MODE_DENSE, 0, full(h)))
     if (c.up && c.host == in) v.push_back(c);
@@ -527,6 +535,10 @@ int rbt_upload(rbt_handle* h, int which, const double* host, void* stream) {
     RBT_CUDA(h, h->d_cpos.ensure(size_t(h->batch) * h->n_grid_max * 3 * h->S.ncon));
     h->cpos_set = true;
   }
+  if (which == RBT_BUF_Q0) {
+    RBT_CUDA(h, h->d_q0.ensure(size_t(h->batch) * h->S.nq));
+    h->q0_set = true;
+  }
   const double* in[N_IN] = {};
   in[d.in] = host;
   return issue(h, upload_plan(h, d.in), true, in, nullptr, (cudaStream_t)stream, "rbt_upload");
@@ -535,8 +547,9 @@ int rbt_upload(rbt_handle* h, int which, const double* host, void* stream) {
 int rbt_download(rbt_handle* h, int which, double* host, void* stream) {
   if (!h || !host) return RBT_ERR_ARG;
   const BufDesc d = buf(h, which);
-  if (which == RBT_BUF_CONTACT_POS && h->stage_ready && !d.ptr) {
-    h->err = "[rbt_download] RBT_BUF_CONTACT_POS has not been uploaded yet";
+  if ((which == RBT_BUF_CONTACT_POS || which == RBT_BUF_Q0) && h->stage_ready && !d.ptr) {
+    h->err = std::string("[rbt_download] ") + (which == RBT_BUF_Q0 ? "RBT_BUF_Q0" : "RBT_BUF_CONTACT_POS") +
+             " has not been uploaded yet";
     return RBT_ERR_STATE;
   }
   if (!d.ptr) return RBT_ERR_ARG;
@@ -1183,6 +1196,25 @@ int rbt_linearize_contact_kinematics(rbt_handle* h, void* stream) {
   return contact_kinematics(h, full(h), (cudaStream_t)stream);
 }
 
+static int state_equation(rbt_handle* h, Win w, cudaStream_t st) {
+  constexpr int NW = rbt::StateCfg::NW;
+  const unsigned n = unsigned((size_t(w.nb) * h->n_grid + NW - 1) / NW);
+  rbt::linearize_state_equation_kernel<CNV><<<n, 32 * NW, 0, st>>>(make_stage_params(h, w), h->d_q0.get() + size_t(w.b0) * h->S.nq,
+                                                                   ctrl_has_sto(h->ctrl.data(), h->n_grid));
+  RBT_CUDA(h, cudaGetLastError());
+  h->launches += 1;
+  return RBT_OK;
+}
+
+int rbt_linearize_state_equation(rbt_handle* h, void* stream) {
+  RBT_STAGE_CHECK(h, "rbt_linearize_state_equation");
+  if (!h->q0_set) {
+    h->err = "[rbt_linearize_state_equation] upload RBT_BUF_Q0 first";
+    return RBT_ERR_STATE;
+  }
+  return state_equation(h, full(h), (cudaStream_t)stream);
+}
+
 int rbt_initial_state_direction(rbt_handle* h, const double* dq0_v0_host, void* stream) {
   RBT_STAGE_CHECK(h, "rbt_initial_state_direction");
   if (!dq0_v0_host) return RBT_ERR_ARG;
@@ -1325,6 +1357,10 @@ static int iteration_host_impl(rbt_handle* h, const double* wire_host, const dou
         return RBT_ERR_STATE;
       }
     }
+    if ((h->cost_structure & RBT_WIRE_DEVICE_STATE) && !h->q0_set) {
+      h->err = "[rbt_iteration_host_wire] the wire records leave the state equation to the device: upload RBT_BUF_Q0 first";
+      return RBT_ERR_STATE;
+    }
     if (sw && !lin_host) {
       h->err = "[rbt_iteration_host_wire] invalid argument: the schedule has switching-constraint stages, their sections come from lin_host_switching";
       return RBT_ERR_ARG;
@@ -1387,6 +1423,7 @@ static int iteration_host_impl(rbt_handle* h, const double* wire_host, const dou
       h->launches += 1;
       if ((h->cost_structure & RBT_WIRE_DEVICE_ID) && (rc = inverse_dynamics(h, w, st))) return rc;
       if ((h->cost_structure & RBT_WIRE_DEVICE_CONTACT) && (rc = contact_kinematics(h, w, st))) return rc;
+      if ((h->cost_structure & RBT_WIRE_DEVICE_STATE) && (rc = state_equation(h, w, st))) return rc;
     }
     if ((rc = condense(h, w, st)) || (rc = backward(h, 0, w, st)) || (rc = forward(h, w, st)) || (rc = expand(h, w, st)) ||
         (rc = update(h, w, st)))
@@ -1426,7 +1463,8 @@ int rbt_iteration_host_resident(rbt_handle* h, const double* wire_host, const do
 }
 
 int rbt_set_wire_cost_structure(rbt_handle* h, int cost_structure) {
-  if (!h || (cost_structure & ~(RBT_COST_ROBOTOC | RBT_WIRE_DEVICE_ID | RBT_WIRE_DEVICE_CONTACT)) != 0) return RBT_ERR_ARG;
+  if (!h || (cost_structure & ~(RBT_COST_ROBOTOC | RBT_WIRE_DEVICE_ID | RBT_WIRE_DEVICE_CONTACT | RBT_WIRE_DEVICE_STATE)) != 0)
+    return RBT_ERR_ARG;
   if (h->cost_structure != cost_structure) h->wire_dirty = true;
   h->cost_structure = cost_structure;
   return RBT_OK;

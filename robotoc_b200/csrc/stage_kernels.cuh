@@ -1125,6 +1125,100 @@ __device__ __forceinline__ void integrate_free_flyer_dev(double* q, const double
   q[3] = nx_ * nrm; q[4] = ny * nrm; q[5] = nz * nrm; q[6] = nw * nrm;
 }
 
+// Free-flyer part of pinocchio::difference(q0, q1) = log6(M0^-1 M1), q = [p | x y z w], motion = [linear | angular].  The
+// rotation comes from the relative quaternion e = conj(quat0) (x) quat1, re-signed to w >= 0: th = 2 atan2(|e_v|, e_w) lies in
+// [0, pi] and needs no arccos (exact at th = 0 and well conditioned at pi).  Writes xi = log6(M), M's rotation R (column-major)
+// and translation p = R0^T (p1 - p0), and coef = {alpha, beta, beta'(th) / th} for se3_jlog6_dev:
+//   alpha = (th / 2) cot(th / 2),  beta = (1 - alpha) / th^2,  v = alpha p - w x p / 2 + beta (w . p) w.
+// Below th = 0.1 the three coefficients are Taylor series in th^2 (their closed forms cancel there); tests/state_ref.py
+// restates this function operation for operation.
+__device__ __forceinline__ void se3_log6_dev(const double* q0, const double* q1, double* xi, double* R, double* p, double* coef) {
+  const double ax = q0[3], ay = q0[4], az = q0[5], aw = q0[6], bx = q1[3], by = q1[4], bz = q1[5], bw = q1[6];
+  double ex = aw * bx - ax * bw - ay * bz + az * by, ey = aw * by + ax * bz - ay * bw - az * bx;
+  double ez = aw * bz - ax * by + ay * bx - az * bw, ew = aw * bw + ax * bx + ay * by + az * bz;
+  if (ew < 0.0) { ex = -ex; ey = -ey; ez = -ez; ew = -ew; }
+  const double s = sqrt(ex * ex + ey * ey + ez * ez);
+  const double ratio = s < 1e-6 ? 2.0 / ew * (1.0 - s * s / (3.0 * ew * ew)) : 2.0 * atan2(s, ew) / s;
+  const double wx = ratio * ex, wy = ratio * ey, wz = ratio * ez, th = ratio * s;
+  {  // p = R(quat0)^T (p1 - p0) = d - 2 w0 (v0 x d) + 2 v0 x (v0 x d)
+    const double dx = q1[0] - q0[0], dy = q1[1] - q0[1], dz = q1[2] - q0[2];
+    const double ux = ay * dz - az * dy, uy = az * dx - ax * dz, uz = ax * dy - ay * dx;
+    p[0] = dx - 2.0 * aw * ux + 2.0 * (ay * uz - az * uy);
+    p[1] = dy - 2.0 * aw * uy + 2.0 * (az * ux - ax * uz);
+    p[2] = dz - 2.0 * aw * uz + 2.0 * (ax * uy - ay * ux);
+  }
+  double alpha, beta, bdot;
+  if (th < 0.1) {
+    const double t = th * th;
+    alpha = 1.0 - t * (1.0 / 12 + t * (1.0 / 720 + t * (1.0 / 30240 + t * (1.0 / 1209600))));
+    beta = 1.0 / 12 + t * (1.0 / 720 + t * (1.0 / 30240 + t * (1.0 / 1209600 + t * (1.0 / 47900160))));
+    bdot = 1.0 / 360 + t * (1.0 / 7560 + t * (1.0 / 201600 + t * (1.0 / 5987520)));
+  } else {
+    const double t = th * th;
+    double sh, ch;
+    sincos(0.5 * th, &sh, &ch);
+    alpha = 0.5 * th * ch / sh;
+    beta = (1.0 - alpha) / t;
+    bdot = -2.0 / (t * t) + (1.0 + 2.0 * sh * ch / th) / (t * 4.0 * sh * sh);
+  }
+  coef[0] = alpha; coef[1] = beta; coef[2] = bdot;
+  const double wp = wx * p[0] + wy * p[1] + wz * p[2];
+  xi[0] = alpha * p[0] - 0.5 * (wy * p[2] - wz * p[1]) + beta * wp * wx;
+  xi[1] = alpha * p[1] - 0.5 * (wz * p[0] - wx * p[2]) + beta * wp * wy;
+  xi[2] = alpha * p[2] - 0.5 * (wx * p[1] - wy * p[0]) + beta * wp * wz;
+  xi[3] = wx; xi[4] = wy; xi[5] = wz;
+  // R(e) = I + 2 e_w [e_v]x + 2 [e_v]x^2
+  R[0] = 1.0 - 2.0 * (ey * ey + ez * ez); R[3] = 2.0 * (ex * ey - ez * ew);       R[6] = 2.0 * (ex * ez + ey * ew);
+  R[1] = 2.0 * (ex * ey + ez * ew);       R[4] = 1.0 - 2.0 * (ex * ex + ez * ez); R[7] = 2.0 * (ey * ez - ex * ew);
+  R[2] = 2.0 * (ex * ez - ey * ew);       R[5] = 2.0 * (ey * ez + ex * ew);       R[8] = 1.0 - 2.0 * (ex * ex + ey * ey);
+}
+
+// pinocchio::Jlog6(M) (column-major 6x6) from se3_log6_dev's xi, p and coef: [[A, C A], [0, A]] with
+//   A = Jlog3 = alpha I + [w]x / 2 + beta w w^T,
+//   C = ((beta' / th)(w . p) w - (th^2 beta' / th + 2 beta) p) w^T + beta w p^T + beta (w . p) I + [p]x / 2.
+// dDifference: ARG1 = Jlog6(M), ARG0 = -Jlog6(M) Ad(M^-1).
+__device__ __forceinline__ void se3_jlog6_dev(const double* xi, const double* p, const double* coef, double* J) {
+  const double alpha = coef[0], beta = coef[1], bdot = coef[2];
+  const double w[3] = {xi[3], xi[4], xi[5]};
+  const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2], wp = w[0] * p[0] + w[1] * p[1] + w[2] * p[2];
+  const double u[3] = {bdot * wp * w[0] - (th2 * bdot + 2.0 * beta) * p[0], bdot * wp * w[1] - (th2 * bdot + 2.0 * beta) * p[1],
+                       bdot * wp * w[2] - (th2 * bdot + 2.0 * beta) * p[2]};
+  double A[9], C[9];
+  for (int c = 0; c < 3; ++c)
+    for (int r = 0; r < 3; ++r) {
+      const int e = r + 3 * c;
+      // [x]x (r, c) = -eps_rck x_k: (1,0) = x2, (0,1) = -x2, (2,0) = -x1, (0,2) = x1, (2,1) = x0, (1,2) = -x0
+      const int k = 3 - r - c;
+      const double sgn = (r == c) ? 0.0 : (((c - r + 3) % 3 == 1) ? -1.0 : 1.0);
+      A[e] = (r == c ? alpha : 0.0) + (r == c ? 0.0 : 0.5 * sgn * w[k]) + beta * w[r] * w[c];
+      C[e] = u[r] * w[c] + beta * w[r] * p[c] + (r == c ? wp * beta : 0.0) + (r == c ? 0.0 : 0.5 * sgn * p[k]);
+    }
+  for (int c = 0; c < 6; ++c)
+    for (int r = 0; r < 6; ++r) {
+      double v = 0.0;
+      if (r < 3 && c < 3) v = A[r + 3 * c];
+      else if (r >= 3 && c >= 3) v = A[(r - 3) + 3 * (c - 3)];
+      else if (r < 3) v = C[r] * A[3 * (c - 3)] + C[r + 3] * A[1 + 3 * (c - 3)] + C[r + 6] * A[2 + 3 * (c - 3)];
+      J[r + 6 * c] = v;
+    }
+}
+
+// Ad(M^-1) (column-major 6x6) of M = (R, p) on motions [linear | angular]: [[R^T, -R^T [p]x], [0, R^T]]
+__device__ __forceinline__ void se3_ad_inv_dev(const double* R, const double* p, double* Ad) {
+  for (int c = 0; c < 6; ++c)
+    for (int r = 0; r < 6; ++r) {
+      double v = 0.0;
+      if ((r < 3) == (c < 3)) {
+        v = R[(c % 3) + 3 * (r % 3)];
+      } else if (r < 3) {  // -(R^T [p]x)(r, c') = -sum_k R(k, r) [p]x(k, c')
+        const int cc = c - 3;
+        const double px[9] = {0.0, p[2], -p[1], -p[2], 0.0, p[0], p[1], -p[0], 0.0};  // [p]x column-major
+        v = -(R[3 * r] * px[3 * cc] + R[1 + 3 * r] * px[1 + 3 * cc] + R[2 + 3 * r] * px[2 + 3 * cc]);
+      }
+      Ad[r + 6 * c] = v;
+    }
+}
+
 #ifndef RBT_UPD_MIN_CTAS
 #define RBT_UPD_MIN_CTAS 8  // 64 registers (48 B of spills); measured faster than 6 CTAs/SM without spills and than 10 or 12
 #endif

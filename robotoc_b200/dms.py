@@ -16,10 +16,11 @@ import numpy as np
 from .riccati import RiccatiRecursion, _check, _vp
 from .stage import StageDims, StageLayout
 
-LIN, CON, EXP, SOL, XDIR, STEPS, PERF, CONTACT_POS = 6, 7, 8, 9, 10, 11, 12, 13
+LIN, CON, EXP, SOL, XDIR, STEPS, PERF, CONTACT_POS, Q0 = 6, 7, 8, 9, 10, 11, 12, 13, 14
 RBT_MAX_BODIES, RBT_MAX_CONTACTS = 32, 8
 WIRE_DEVICE_ID = 2  # RBT_WIRE_DEVICE_ID (rbt_stage_layout.h)
 WIRE_DEVICE_CONTACT = 4  # RBT_WIRE_DEVICE_CONTACT
+WIRE_DEVICE_STATE = 16  # RBT_WIRE_DEVICE_STATE
 
 
 class rbt_robot_model(ctypes.Structure):
@@ -120,6 +121,23 @@ class DirectMultipleShooting:
         la | ldv, from the resident solution records (setRobotModel, setContactGains and setContactPositions first)."""
         _check(self._lib.rbt_linearize_contact_kinematics(self._h, stream), self.rr._err, "DirectMultipleShooting")
 
+    def setInitialConfiguration(self, q0, stream=None):
+        """The measured configuration q0 [batch, nq] of OCPSolver::solve(t, q, v): grid point 0's q_prev in linearizeStateEquation
+        and the device-side state-equation rows of the wire paths.  Resident: upload again with each new measurement."""
+        q0 = np.ascontiguousarray(q0, dtype=np.float64)
+        shape = (self.rr.batch, self.layout.nq)
+        if q0.shape != shape:
+            raise ValueError(f"[DirectMultipleShooting] invalid argument: q0 must have shape {shape}")
+        _check(self._lib.rbt_upload(self._h, Q0, _vp(q0), stream), self.rr._err, "DirectMultipleShooting")
+        self.rr.synchronize(stream)
+
+    def linearizeStateEquation(self, stream=None):
+        """The state-equation rows of linearizeStateEquation / linearizeImpactStateEquation / linearizeTerminalStateEquation on
+        the device (rbt_linearize_state_equation): Fx, the three SE(3) blocks, the costate terms of lq, lv, la | ldv and, on
+        schedules with a switching-time stage, the STO terms, from the resident solution records (setInitialConfiguration
+        first)."""
+        _check(self._lib.rbt_linearize_state_equation(self._h, stream), self.rr._err, "DirectMultipleShooting")
+
     def computeStepSizes(self, stream=None):
         _check(self._lib.rbt_expand_and_step_sizes(self._h, stream), self.rr._err, "DirectMultipleShooting")
 
@@ -193,16 +211,19 @@ class DirectMultipleShooting:
         return h2d.value, d2h.value
 
     def setWireCostStructure(self, robotoc_costs: bool, device_inverse_dynamics: bool = False,
-                             device_contact_kinematics: bool = False):
+                             device_contact_kinematics: bool = False, device_state_equation: bool = False):
         """Which cost-Hessian structure the host's wire records have: False = general (full packed triangles of Qxx, Quu, Qff),
         True = what robotoc's shipped cost components produce (Qqq dense, Qvv / Quu / Qff diagonal, Qqv = 0).
         device_inverse_dynamics: the wire records leave out M and the ID rows of dIDCdqv and IDC (and their gradients the beta
         terms); iteration_host_wire / iteration_host_resident compute them on the device (setRobotModel first).
         device_contact_kinematics: the wire records leave out J and the contact rows of dIDCdqv and IDC (and their gradients
         the multiplier terms of those rows); the wire paths compute them on the device (setRobotModel, setContactGains and
-        setContactPositions first)."""
+        setContactPositions first).
+        device_state_equation: the wire records leave out Fx and the SE(3) blocks (and their gradients and STO sections the
+        costate terms); the wire paths compute them on the device (setInitialConfiguration first)."""
         self._cost_structure = ((1 if robotoc_costs else 0) | (WIRE_DEVICE_ID if device_inverse_dynamics else 0)
-                                | (WIRE_DEVICE_CONTACT if device_contact_kinematics else 0))
+                                | (WIRE_DEVICE_CONTACT if device_contact_kinematics else 0)
+                                | (WIRE_DEVICE_STATE if device_state_equation else 0))
         _check(self._lib.rbt_set_wire_cost_structure(self._h, self._cost_structure), self.rr._err, "DirectMultipleShooting")
 
     def pack_wire(self, lin):
