@@ -14,7 +14,8 @@
 // registers (q (+) eps e_k = integrate(q, eps e_k), as in rnea_kernels.cuh).  The v-tangent of v_f,lin is the column k of the
 // contact Jacobian J_lin, which is also dC/da on Intermediate / Lift and dC/dv on Impact grid points.
 #pragma once
-#include "rnea_kernels.cuh"
+#include "spatial.cuh"
+#include "stage_kernels.cuh"  // StageParams
 
 namespace rbt {
 
@@ -24,39 +25,6 @@ struct ContactCfg {
   static constexpr int NTHR = 96;  // >= 3 NV + 3 RBT_MAX_CONTACTS: the gradient lanes of the last phase
   static constexpr int NFM = 3 * RBT_MAX_CONTACTS;
 };
-
-// liMi = placement * M_J(q) of body b (R column-major)
-__device__ __forceinline__ void joint_placement(const RneaModel& m, const double* q, int b, double* R, double* p) {
-  double RJ[9], pJ[3] = {0.0, 0.0, 0.0};
-  if (b == 0) {  // free flyer: q = [p | x y z w]
-    const double x = q[3], y = q[4], z = q[5], w = q[6];
-    RJ[0] = 1 - 2 * (y * y + z * z); RJ[3] = 2 * (x * y - z * w);     RJ[6] = 2 * (x * z + y * w);
-    RJ[1] = 2 * (x * y + z * w);     RJ[4] = 1 - 2 * (x * x + z * z); RJ[7] = 2 * (y * z - x * w);
-    RJ[2] = 2 * (x * z - y * w);     RJ[5] = 2 * (y * z + x * w);     RJ[8] = 1 - 2 * (x * x + y * y);
-    pJ[0] = q[0]; pJ[1] = q[1]; pJ[2] = q[2];
-  } else {  // revolute about the unit axis u: Rodrigues
-    double sn, cs;
-    sincos(q[b + 6], &sn, &cs);
-    const double ux = m.axis[b][0], uy = m.axis[b][1], uz = m.axis[b][2], t = 1.0 - cs;
-    RJ[0] = cs + ux * ux * t;      RJ[3] = ux * uy * t - uz * sn; RJ[6] = ux * uz * t + uy * sn;
-    RJ[1] = uy * ux * t + uz * sn; RJ[4] = cs + uy * uy * t;      RJ[7] = uy * uz * t - ux * sn;
-    RJ[2] = uz * ux * t - uy * sn; RJ[5] = uz * uy * t + ux * sn; RJ[8] = cs + uz * uz * t;
-  }
-  const double* RP = m.R[b];
-  for (int j = 0; j < 3; ++j) rot_mul(RP, RJ + 3 * j, R + 3 * j);
-  rot_mul(RP, pJ, p);
-  for (int r = 0; r < 3; ++r) p[r] += m.p[b][r];
-}
-
-// joint motion subspace column k of body b, as joint_s, with every entry selected rather than indexed (registers, no stack)
-__device__ __forceinline__ void joint_s_reg(const RneaModel& m, int b, int k, double* s) {
-  for (int r = 0; r < 6; ++r) s[r] = b == 0 ? (r == k ? 1.0 : 0.0) : (r < 3 ? 0.0 : m.axis[b][r - 3]);
-}
-// joint velocity S qd of body b
-__device__ __forceinline__ void joint_motion(const RneaModel& m, int b, const double* qd, double* vJ) {
-  if (b == 0) { for (int r = 0; r < 6; ++r) vJ[r] = qd[r]; }
-  else { for (int r = 0; r < 3; ++r) { vJ[r] = 0.0; vJ[3 + r] = m.axis[b][r] * qd[b + 5]; } }
-}
 
 // One CTA per (OCP, grid point).  Phase 1: joint placements (one body per lane) and the chain of every active contact.
 // Phase 2: one lane per active contact walks its chain: v, a (no gravity) and the world placement, then the contact frame and
@@ -107,15 +75,9 @@ __global__ void __launch_bounds__(ContactCfg<NV>::NTHR)
     double oR[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0}, op[3] = {0.0, 0.0, 0.0};
     for (int j = 0; j < depth; ++j) {
       const int b = schain[a][j];
-      double vJ[6], w[6], t[3];
-      joint_motion(m, b, sqd, vJ);
-      motion_act_inv(sR[b], sp[b], v, w);
-      for (int r = 0; r < 6; ++r) v[r] = w[r] + vJ[r];
-      motion_act_inv(sR[b], sp[b], acc, w);
-      if (b == 0) { for (int r = 0; r < 6; ++r) w[r] += sqdd[r]; }
-      else { for (int r = 0; r < 3; ++r) w[3 + r] += m.axis[b][r] * sqdd[b + 5]; }
-      motion_cross_add(v, vJ, w);
-      for (int r = 0; r < 6; ++r) { acc[r] = w[r]; sv[a][j][r] = v[r]; sa[a][j][r] = acc[r]; }
+      double t[3];
+      forward_step(m, b, sR[b], sp[b], sqd, sqdd, v, acc, v, acc);
+      for (int r = 0; r < 6; ++r) { sv[a][j][r] = v[r]; sa[a][j][r] = acc[r]; }
       // oMi = oMparent * liMi
       rot_mul(oR, sp[b], t);
       for (int r = 0; r < 3; ++r) op[r] += t[r];
@@ -152,7 +114,7 @@ __global__ void __launch_bounds__(ContactCfg<NV>::NTHR)
       double s[6], vJ[6], w[6];
       double tvq[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, taq[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
       double tvv[6], tav[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-      joint_s_reg(m, jb, k, s);
+      joint_s(m, jb, k, s);
       joint_motion(m, jb, sqd, vJ);
       if (pos > 0) {  // d/deps exp(-eps s) X^-1 m = (X^-1 m) x s, for m = v_parent and a_parent (the root's are zero)
         motion_act_inv(sR[jb], sp[jb], sv[a][pos - 1], w);

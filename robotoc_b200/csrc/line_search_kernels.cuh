@@ -6,7 +6,8 @@
 // evalOCP at the trial points (costs, dynamics residuals) needs the robot model and stays with the host / a GPU front-end; of
 // its PerformanceIndex only the log-barrier of the trial slacks is computed here.
 #pragma once
-#include "stage_kernels.cuh"
+#include "spatial.cuh"        // integrate_free_flyer_dev
+#include "stage_kernels.cuh"  // StageParams
 
 namespace rbt {
 

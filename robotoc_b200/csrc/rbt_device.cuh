@@ -157,19 +157,8 @@ __device__ __forceinline__ void matvec_T(const double* A, int lda, int K, int C,
   }
 }
 
-// y[r] = sum_k A[r + k*lda] * x[k]  (A x), one thread per row (conflict-free: consecutive lanes, consecutive rows).
-template <class Epi>
-__device__ __forceinline__ void matvec_N(const double* A, int lda, int R, int K, const double* x, int tid, int nthr,
-                                         Epi epi) {
-  for (int r = tid; r < R; r += nthr) {
-    double acc = 0.0;
-    for (int k = 0; k < K; ++k) acc = fma(A[r + k * lda], x[k], acc);
-    epi(r, acc);
-  }
-}
-
 // y[r] = sum_k A[r + k*lda] * x[k]  (A x) with 4 lanes per row (k interleaved) + 2 shuffles: 4x shorter dependent chain
-// than matvec_N.  Call with whole warps (nthr multiple of 32).
+// than one thread per row.  Call with whole warps (nthr multiple of 32).
 template <class Epi>
 __device__ __forceinline__ void matvec_N4(const double* A, int lda, int R, int K, const double* x, int tid, int nthr,
                                           Epi epi) {
@@ -244,6 +233,15 @@ __device__ __forceinline__ bool warp_chol_inv_reg(double (&c)[N], double& rs) {
 #pragma unroll
   for (int j = 0; j < N; ++j) c[j] *= __shfl_sync(0xffffffffu, rs, j);  // L[r][j] = a_rj / sqrt(d_j) | (L^-1)[j][q] = e_j[q] / sqrt(d_j)
   return ok;
+}
+
+__device__ __forceinline__ double warp_min(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ void atomic_min_pos(double* addr, double v) {  // v > 0: IEEE order == unsigned integer order
+  atomicMin(reinterpret_cast<unsigned long long*>(addr), static_cast<unsigned long long>(__double_as_longlong(v)));
 }
 
 // Not unrolled: the chain is serial anyway, and with a compile-time n the unrolled loop hoists all 2n loads, which spilled

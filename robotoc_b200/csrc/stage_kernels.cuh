@@ -17,6 +17,7 @@
 #pragma once
 #include "rbt_device.cuh"
 #include "riccati_backward.cuh"  // warp_cholesky, chol_solve_smem
+#include "spatial.cuh"           // integrate_free_flyer_dev, se3_jac_inverse_dev
 #include "../../include/rbt_stage_layout.h"
 
 namespace rbt {
@@ -42,52 +43,6 @@ struct StageParams {
                     // (row + 1) * sign of the row, 0 = none
   const int* row_level;  // [n_box] 2 = position-, 1 = velocity-, 0 = acceleration-level row: acts iff level + ctrl.ineq_gate <= 2
 };
-
-// C(m x n, ld ldc) = beta*C + alpha * op(A) op(B); all operands in shared (or global) memory; every thread of the CTA calls.
-__device__ __forceinline__ void cta_gemm(int ta, int tb, int m, int n, int k, double alpha, const double* A, int lda,
-                                         const double* B, int ldb, double beta, double* C, int ldc) {
-  for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
-    const int i = e % m, j = e / m;
-    double acc = 0.0;
-    for (int l = 0; l < k; ++l) {
-      const double a = ta ? A[l + i * lda] : A[i + l * lda];
-      const double b = tb ? B[j + l * ldb] : B[l + j * ldb];
-      acc = fma(a, b, acc);
-    }
-    const double c0 = (beta == 0.0) ? 0.0 : beta * C[i + j * ldc];
-    C[i + j * ldc] = fma(alpha, acc, c0);
-  }
-}
-
-__device__ __forceinline__ void inv3_dev(const double* A, int lda, double* B, int ldb) {
-  const double a = A[0], b = A[lda], c = A[2 * lda], d = A[1], e = A[1 + lda], f = A[1 + 2 * lda], g = A[2], h = A[2 + lda],
-               i = A[2 + 2 * lda];
-  const double det = a * (e * i - f * h) - b * (d * i - f * g) + c * (d * h - e * g);
-  const double r = 1.0 / det;
-  B[0] = (e * i - f * h) * r; B[ldb] = (c * h - b * i) * r; B[2 * ldb] = (b * f - c * e) * r;
-  B[1] = (f * g - d * i) * r; B[1 + ldb] = (a * i - c * g) * r; B[1 + 2 * ldb] = (c * d - a * f) * r;
-  B[2] = (d * h - e * g) * r; B[2 + ldb] = (b * g - a * h) * r; B[2 + 2 * ldb] = (a * e - b * d) * r;
-}
-
-// SE3JacobianInverse::compute (se3_jacobian_inverse.hxx:17-32); one thread; Jac may be global, Jinv shared/global (ld 6)
-__device__ __noinline__ void se3_jac_inverse_dev(const double* Jac, double* Jinv) {
-  double tmp[9];
-  for (int q = 0; q < 36; ++q) Jinv[q] = 0.0;
-  inv3_dev(Jac, 6, Jinv, 6);
-  inv3_dev(Jac + 3 + 18, 6, Jinv + 3 + 18, 6);
-  for (int j = 0; j < 3; ++j)
-    for (int i = 0; i < 3; ++i) {
-      double acc = 0.0;
-      for (int l = 0; l < 3; ++l) acc = fma(Jac[i + (3 + l) * 6], Jinv[(3 + l) + (3 + j) * 6], acc);
-      tmp[i + 3 * j] = acc;
-    }
-  for (int j = 0; j < 3; ++j)
-    for (int i = 0; i < 3; ++i) {
-      double acc = 0.0;
-      for (int l = 0; l < 3; ++l) acc = fma(Jinv[i + l * 6], tmp[l + 3 * j], acc);
-      Jinv[i + (3 + j) * 6] = -acc;
-    }
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 // K1: Z = [[M, J^T],[J, 0]]^-1  (Robot::computeMJtJinv, include/robotoc/robot/robot.hxx:642-683, dense restatement)
@@ -961,15 +916,6 @@ __global__ void __launch_bounds__(64) pack_slack_dual_kernel(const double* con, 
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double warp_min(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ void atomic_min_pos(double* addr, double v) {  // v > 0: IEEE order == unsigned integer order
-  atomicMin(reinterpret_cast<unsigned long long*>(addr), static_cast<unsigned long long>(__double_as_longlong(v)));
-}
-
 // expand / update: one CTA of 4 warps per (OCP, stage).  The matrices of the expansion record arrive in shared memory by
 // TMA bulk copies (one round trip to HBM instead of a chain of dependent column loads); each warp then owns every 4th
 // column of a mat-vec (lane = row, conflict-free) and the partial sums meet in shared memory.
@@ -1091,132 +1037,6 @@ __global__ void __launch_bounds__(XTHR, RBT_EXP_MIN_CTAS) expand_kernel(const St
     atomic_min_pos(&p.steps[2 * b], fmin(fmin(smin[0], smin[2]), fmin(smin[4], smin[6])));
     atomic_min_pos(&p.steps[2 * b + 1], fmin(fmin(smin[1], smin[3]), fmin(smin[5], smin[7])));
   }
-}
-
-// free-flyer part of Robot::integrateConfiguration (textbook SE(3) exponential; see oracle/condense_oracle.c)
-__device__ __forceinline__ void integrate_free_flyer_dev(double* q, const double* dq, double step) {
-  const double vx = step * dq[0], vy = step * dq[1], vz = step * dq[2];
-  const double wx = step * dq[3], wy = step * dq[4], wz = step * dq[5];
-  const double th2 = wx * wx + wy * wy + wz * wz, th = sqrt(th2);
-  double bb, cc, s2 = 0.0, c2 = 1.0;  // one sincos of the half angle serves both the translation and the quaternion part
-  if (th < 1e-6) {
-    bb = 0.5 - th2 / 24.0; cc = 1.0 / 6.0 - th2 / 120.0;
-  } else {
-    sincos(0.5 * th, &s2, &c2);
-    bb = 2.0 * s2 * s2 / th2; cc = (th - 2.0 * s2 * c2) / (th2 * th);
-  }
-  const double cx = wy * vz - wz * vy, cy = wz * vx - wx * vz, cz = wx * vy - wy * vx;
-  const double ccx = wy * cz - wz * cy, ccy = wz * cx - wx * cz, ccz = wx * cy - wy * cx;
-  const double tx = vx + bb * cx + cc * ccx, ty = vy + bb * cy + cc * ccy, tz = vz + bb * cz + cc * ccz;
-  const double qx = q[3], qy = q[4], qz = q[5], qw = q[6];
-  const double ux = qy * tz - qz * ty, uy = qz * tx - qx * tz, uz = qx * ty - qy * tx;
-  const double u2x = qy * uz - qz * uy, u2y = qz * ux - qx * uz, u2z = qx * uy - qy * ux;
-  q[0] += tx + 2.0 * (qw * ux + u2x);
-  q[1] += ty + 2.0 * (qw * uy + u2y);
-  q[2] += tz + 2.0 * (qw * uz + u2z);
-  double sh, ch;
-  if (th < 1e-6) { sh = 0.5 - th2 / 48.0; ch = 1.0 - th2 / 8.0; } else { sh = s2 / th; ch = c2; }
-  const double ex_ = sh * wx, ey = sh * wy, ez = sh * wz, ew = ch;
-  const double nx_ = qw * ex_ + qx * ew + qy * ez - qz * ey;
-  const double ny = qw * ey - qx * ez + qy * ew + qz * ex_;
-  const double nz = qw * ez + qx * ey - qy * ex_ + qz * ew;
-  const double nw = qw * ew - qx * ex_ - qy * ey - qz * ez;
-  const double nrm = 1.0 / sqrt(nx_ * nx_ + ny * ny + nz * nz + nw * nw);
-  q[3] = nx_ * nrm; q[4] = ny * nrm; q[5] = nz * nrm; q[6] = nw * nrm;
-}
-
-// Free-flyer part of pinocchio::difference(q0, q1) = log6(M0^-1 M1), q = [p | x y z w], motion = [linear | angular].  The
-// rotation comes from the relative quaternion e = conj(quat0) (x) quat1, re-signed to w >= 0: th = 2 atan2(|e_v|, e_w) lies in
-// [0, pi] and needs no arccos (exact at th = 0 and well conditioned at pi).  Writes xi = log6(M), M's rotation R (column-major)
-// and translation p = R0^T (p1 - p0), and coef = {alpha, beta, beta'(th) / th} for se3_jlog6_dev:
-//   alpha = (th / 2) cot(th / 2),  beta = (1 - alpha) / th^2,  v = alpha p - w x p / 2 + beta (w . p) w.
-// Below th = 0.1 the three coefficients are Taylor series in th^2 (their closed forms cancel there); tests/state_ref.py
-// restates this function operation for operation.
-__device__ __forceinline__ void se3_log6_dev(const double* q0, const double* q1, double* xi, double* R, double* p, double* coef) {
-  const double ax = q0[3], ay = q0[4], az = q0[5], aw = q0[6], bx = q1[3], by = q1[4], bz = q1[5], bw = q1[6];
-  double ex = aw * bx - ax * bw - ay * bz + az * by, ey = aw * by + ax * bz - ay * bw - az * bx;
-  double ez = aw * bz - ax * by + ay * bx - az * bw, ew = aw * bw + ax * bx + ay * by + az * bz;
-  if (ew < 0.0) { ex = -ex; ey = -ey; ez = -ez; ew = -ew; }
-  const double s = sqrt(ex * ex + ey * ey + ez * ez);
-  const double ratio = s < 1e-6 ? 2.0 / ew * (1.0 - s * s / (3.0 * ew * ew)) : 2.0 * atan2(s, ew) / s;
-  const double wx = ratio * ex, wy = ratio * ey, wz = ratio * ez, th = ratio * s;
-  {  // p = R(quat0)^T (p1 - p0) = d - 2 w0 (v0 x d) + 2 v0 x (v0 x d)
-    const double dx = q1[0] - q0[0], dy = q1[1] - q0[1], dz = q1[2] - q0[2];
-    const double ux = ay * dz - az * dy, uy = az * dx - ax * dz, uz = ax * dy - ay * dx;
-    p[0] = dx - 2.0 * aw * ux + 2.0 * (ay * uz - az * uy);
-    p[1] = dy - 2.0 * aw * uy + 2.0 * (az * ux - ax * uz);
-    p[2] = dz - 2.0 * aw * uz + 2.0 * (ax * uy - ay * ux);
-  }
-  double alpha, beta, bdot;
-  if (th < 0.1) {
-    const double t = th * th;
-    alpha = 1.0 - t * (1.0 / 12 + t * (1.0 / 720 + t * (1.0 / 30240 + t * (1.0 / 1209600))));
-    beta = 1.0 / 12 + t * (1.0 / 720 + t * (1.0 / 30240 + t * (1.0 / 1209600 + t * (1.0 / 47900160))));
-    bdot = 1.0 / 360 + t * (1.0 / 7560 + t * (1.0 / 201600 + t * (1.0 / 5987520)));
-  } else {
-    const double t = th * th;
-    double sh, ch;
-    sincos(0.5 * th, &sh, &ch);
-    alpha = 0.5 * th * ch / sh;
-    beta = (1.0 - alpha) / t;
-    bdot = -2.0 / (t * t) + (1.0 + 2.0 * sh * ch / th) / (t * 4.0 * sh * sh);
-  }
-  coef[0] = alpha; coef[1] = beta; coef[2] = bdot;
-  const double wp = wx * p[0] + wy * p[1] + wz * p[2];
-  xi[0] = alpha * p[0] - 0.5 * (wy * p[2] - wz * p[1]) + beta * wp * wx;
-  xi[1] = alpha * p[1] - 0.5 * (wz * p[0] - wx * p[2]) + beta * wp * wy;
-  xi[2] = alpha * p[2] - 0.5 * (wx * p[1] - wy * p[0]) + beta * wp * wz;
-  xi[3] = wx; xi[4] = wy; xi[5] = wz;
-  // R(e) = I + 2 e_w [e_v]x + 2 [e_v]x^2
-  R[0] = 1.0 - 2.0 * (ey * ey + ez * ez); R[3] = 2.0 * (ex * ey - ez * ew);       R[6] = 2.0 * (ex * ez + ey * ew);
-  R[1] = 2.0 * (ex * ey + ez * ew);       R[4] = 1.0 - 2.0 * (ex * ex + ez * ez); R[7] = 2.0 * (ey * ez - ex * ew);
-  R[2] = 2.0 * (ex * ez - ey * ew);       R[5] = 2.0 * (ey * ez + ex * ew);       R[8] = 1.0 - 2.0 * (ex * ex + ey * ey);
-}
-
-// pinocchio::Jlog6(M) (column-major 6x6) from se3_log6_dev's xi, p and coef: [[A, C A], [0, A]] with
-//   A = Jlog3 = alpha I + [w]x / 2 + beta w w^T,
-//   C = ((beta' / th)(w . p) w - (th^2 beta' / th + 2 beta) p) w^T + beta w p^T + beta (w . p) I + [p]x / 2.
-// dDifference: ARG1 = Jlog6(M), ARG0 = -Jlog6(M) Ad(M^-1).
-__device__ __forceinline__ void se3_jlog6_dev(const double* xi, const double* p, const double* coef, double* J) {
-  const double alpha = coef[0], beta = coef[1], bdot = coef[2];
-  const double w[3] = {xi[3], xi[4], xi[5]};
-  const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2], wp = w[0] * p[0] + w[1] * p[1] + w[2] * p[2];
-  const double u[3] = {bdot * wp * w[0] - (th2 * bdot + 2.0 * beta) * p[0], bdot * wp * w[1] - (th2 * bdot + 2.0 * beta) * p[1],
-                       bdot * wp * w[2] - (th2 * bdot + 2.0 * beta) * p[2]};
-  double A[9], C[9];
-  for (int c = 0; c < 3; ++c)
-    for (int r = 0; r < 3; ++r) {
-      const int e = r + 3 * c;
-      // [x]x (r, c) = -eps_rck x_k: (1,0) = x2, (0,1) = -x2, (2,0) = -x1, (0,2) = x1, (2,1) = x0, (1,2) = -x0
-      const int k = 3 - r - c;
-      const double sgn = (r == c) ? 0.0 : (((c - r + 3) % 3 == 1) ? -1.0 : 1.0);
-      A[e] = (r == c ? alpha : 0.0) + (r == c ? 0.0 : 0.5 * sgn * w[k]) + beta * w[r] * w[c];
-      C[e] = u[r] * w[c] + beta * w[r] * p[c] + (r == c ? wp * beta : 0.0) + (r == c ? 0.0 : 0.5 * sgn * p[k]);
-    }
-  for (int c = 0; c < 6; ++c)
-    for (int r = 0; r < 6; ++r) {
-      double v = 0.0;
-      if (r < 3 && c < 3) v = A[r + 3 * c];
-      else if (r >= 3 && c >= 3) v = A[(r - 3) + 3 * (c - 3)];
-      else if (r < 3) v = C[r] * A[3 * (c - 3)] + C[r + 3] * A[1 + 3 * (c - 3)] + C[r + 6] * A[2 + 3 * (c - 3)];
-      J[r + 6 * c] = v;
-    }
-}
-
-// Ad(M^-1) (column-major 6x6) of M = (R, p) on motions [linear | angular]: [[R^T, -R^T [p]x], [0, R^T]]
-__device__ __forceinline__ void se3_ad_inv_dev(const double* R, const double* p, double* Ad) {
-  for (int c = 0; c < 6; ++c)
-    for (int r = 0; r < 6; ++r) {
-      double v = 0.0;
-      if ((r < 3) == (c < 3)) {
-        v = R[(c % 3) + 3 * (r % 3)];
-      } else if (r < 3) {  // -(R^T [p]x)(r, c') = -sum_k R(k, r) [p]x(k, c')
-        const int cc = c - 3;
-        const double px[9] = {0.0, p[2], -p[1], -p[2], 0.0, p[0], p[1], -p[0], 0.0};  // [p]x column-major
-        v = -(R[3 * r] * px[3 * cc] + R[1 + 3 * r] * px[1 + 3 * cc] + R[2 + 3 * r] * px[2 + 3 * cc]);
-      }
-      Ad[r + 6 * c] = v;
-    }
 }
 
 #ifndef RBT_UPD_MIN_CTAS

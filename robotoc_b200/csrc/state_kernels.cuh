@@ -14,9 +14,10 @@
 //   STO terms (schedules with a switching-time stage, Intermediate / Lift only):
 //                        h += lmd_next . v + gmm_next . a,  hv += lmd_next,  ha += gmm_next,  fq = v,  fv = a
 //   Terminal:            Fqq_prev,  lq[0:6] += Fqq_prev^T lmd[0:6],  lq[6:] -= lmd[6:],  lv -= gmm
-// The SE(3) log, Jlog6 and Ad live next to the free-flyer exponential in stage_kernels.cuh.
+// The SE(3) log, Jlog6 and Ad live next to the free-flyer exponential in spatial.cuh.
 #pragma once
-#include "stage_kernels.cuh"
+#include "spatial.cuh"
+#include "stage_kernels.cuh"  // StageParams
 
 namespace rbt {
 

@@ -21,7 +21,6 @@
 // left untouched.
 #pragma once
 #include "rbt_device.cuh"
-#include "stage_kernels.cuh"  // warp_min, atomic_min_pos
 #include "../../include/rbt_ustage_layout.h"
 
 namespace rbt {

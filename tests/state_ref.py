@@ -11,7 +11,7 @@ linearizeTerminalStateEquation (terminal_state_equation.cpp:8-28), with correctL
 The log is taken from the relative quaternion conj(quat0) (x) quat1, re-signed to w >= 0, so the angle is 2 atan2(|v|, w) in
 [0, pi] and needs no arccos.  Jlog3 = alpha I + [w]x / 2 + beta w w^T and Jlog6 = [[Jlog3, C Jlog3], [0, Jlog3]] with
 alpha = (th / 2) cot(th / 2), beta = (1 - alpha) / th^2 and C as in Pinocchio's Jlog6; below th = 0.1 the three scalar
-coefficients come from their Taylor series.  stage_kernels.cuh (se3_log6_dev, se3_jlog6_dev, se3_ad_inv_dev) evaluates the
+coefficients come from their Taylor series.  spatial.cuh (se3_log6_dev, se3_jlog6_dev, se3_ad_inv_dev) evaluates the
 same expressions in the same order; tests/test_state_equation.py pins them by central differences, by round trips through
 rbd_ref.integrate and by a 100-digit matrix log."""
 import numpy as np
